@@ -1,8 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — BASELINE.json's metric on N B200s of one node: denoise-steps/s and images/s of the
-FLUX.1-dev 1024x1024 reflection tree (28 steps x 8 candidates x 4 rounds).
+"""bench.py — denoise-steps/s and images/s of the FLUX.1-dev 1024x1024 reflection tree
+(28 steps x 8 candidates x 4 rounds) on N H100s of one node.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]          product arm (CUDA kernels)
+  python bench.py ... --dump-outputs DIR                        also write the final latents of the
+                                                                timed headline call to DIR/latents.npy
   python bench.py --impl reference ...                          reference arm: the reference's CPU
                                                                 path (oracle port) on host cores
 
@@ -62,12 +64,13 @@ def peaks():
         j = json.load(open(p))
         return {"tflops_burst": j["bf16_tflops"], "tflops_sustained": j["bf16_tflops_sustained"],
                 "hbm_gbs": j["hbm_gbs"], "source": "measured"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense bf16, HBM3), not measured: the sustained rate under a power cap is lower
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0,
+            "source": "fallback (H100 SXM data sheet)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -310,6 +313,8 @@ def main():
     ap.add_argument("--no-text", action="store_true", help="tree with hash text embeddings instead of native T5/CLIP")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--layers", default="19,38", help="double,single layer counts (debug only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final latents of the last timed headline call as DIR/latents.npy (float32)")
     args = ap.parse_args()
     K, Wm = max(args.steps, 1), max(args.warmup, 0)
     rank = int(os.environ.get("RANK", "0"))
@@ -320,7 +325,7 @@ def main():
                           f"(lora_mode={args.lora_mode}), guidance 3.5, batch 1, 1 candidate per GPU; `tree` = 8 candidates x 4 "
                           "rounds x --steps denoise steps as one timed call",
               "parallelism": f"candidate-sharded x{args.gpus} (replicated weights)",
-              "l2": "inputs larger than L2: every step streams 23.8 GB of weights (L2 = 126 MB)",
+              "l2": "inputs larger than L2: every step streams 23.8 GB of weights (H100 L2 = 50 MB)",
               "weights": "random-init (seeded), FLUX.1-dev architecture, 11.9 B params bf16 + rank-32 LoRA"}
 
     if args.impl == "reference":
@@ -429,6 +434,11 @@ def main():
     launches = lib.rf_launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
     log(f"headline: {ms / K:.2f} ms/step")
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        # [1, 4096, 64] packed latents: what model.denoise() hands its caller (1 MB as float32)
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), final.float().cpu().numpy())
 
     # ---- e2e: the public API call (generate(), entry B) with HOST inputs and a host read-back
     def e2e_call(n):
@@ -589,23 +599,16 @@ def main():
     step_tflop = algorithmic_tflop(n_tok, nl + ns)
     step_tflop_a = algorithmic_tflop(N_TXT + N_IMG, nl + ns)
     steps_per_s = args.gpus * K / (ms / 1e3)
-    # the LoRA down-projections run on a forked stream, on two reserved TPCs, UNDER the other streams' GEMMs
+    # the LoRA down-projections run on a forked stream, on a few reserved SMs, beside the other streams' GEMMs
     # (csrc/dit.cu): their launch durations overlap those GEMMs and are not part of the step's critical path
     forked = {"lora_down"} if (args.lora_mode == "exact" and os.environ.get("RF_SIDE_STREAM", "1") != "0") else set()
     tot_ms = sum(v["ms"] for k, v in prof.items() if k not in forked)
     dom_name, dom = max(((k, v) for k, v in prof.items() if k not in forked), key=lambda kv: kv[1]["ms"])
     ach = dom["flops"] / (dom["ms"] / 1e3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get(dom_name)
     roofline = {"kernel": dom_name, "bound": "tensor", "achieved": ach,
                 "peak": pk["tflops_sustained"], "unit": "TFLOP/s", "frac": ach / pk["tflops_sustained"],
-                "peak_source": pk["source"] + " (sustained cuBLAS bf16: the kernel is timed inside a long step)",
-                "traffic": traffic,
-                "traffic_note": "DRAM bytes per launch (launch-weighted over the kernel's shapes) from the committed "
-                                "ncu --set full capture (profiles/ncu_traffic.json); algorithmic bytes per launch = "
-                                + str(round(dom["bytes"] / dom["launches"])),
+                "peak_source": pk["source"],
+                "algorithmic_bytes_per_launch": round(dom["bytes"] / dom["launches"]),
                 "launches_per_step": dom["launches"], "avg_launch_ms": dom["ms"] / dom["launches"],
                 "share_of_step": dom["ms"] / tot_ms,
                 "how": "CUDA events around every launch of one eager headline forward inside this run"}
@@ -614,7 +617,7 @@ def main():
                    "tflops": round(v["flops"] / (v["ms"] / 1e3) / 1e12, 1) if v["flops"] else None,
                    "gbs": round(v["bytes"] / (v["ms"] / 1e3) / 1e9, 1)} for k, v in prof.items()}
     for k in forked & set(kernels):
-        kernels[k]["note"] = ("forked stream: 4 CTAs on two reserved TPCs, concurrent with the image + text GEMM of the "
+        kernels[k]["note"] = ("forked stream: 4 CTAs on reserved SMs, concurrent with the image + text GEMM of the "
                               "same layer; its duration is hidden, not a share of the step")
     line = {"metric": "denoise-steps/sec", "value": steps_per_s, "unit": "denoise-steps/s",
             "n_gpus": args.gpus, "steps": K, "warmup": Wm, "ms_per_step": ms / K,

@@ -5,7 +5,7 @@
  *   gcc -std=c11 -O2 -Iinclude -I/usr/local/cuda/include examples/c_abi_linear.c \
  *       -Lreflectionflow_b200 -lrf_b200 -L/usr/local/cuda/lib64 -lcudart -lm \
  *       -Wl,-rpath,$PWD/reflectionflow_b200 -o examples/c_abi_linear
- *   ./examples/c_abi_linear            (needs a B200; exits 2 with the library's message otherwise)
+ *   ./examples/c_abi_linear            (needs an H100; exits 2 with the library's message otherwise)
  */
 #include <cuda_runtime_api.h>
 #include <math.h>

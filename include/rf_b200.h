@@ -1,4 +1,4 @@
-/* rf_b200.h — C ABI of librf_b200.so: the B200-native (sm_100a) FLUX.1-dev DiT hot path of
+/* rf_b200.h — C ABI of librf_b200.so: the H100-native (sm_90a) FLUX.1-dev DiT hot path of
  * Diffusion-CoT/ReflectionFlow.
  *
  * The reference has no FFI layer (it is pure Python over diffusers); its de-facto operator
@@ -59,10 +59,10 @@ int rf_op_linear(int epilogue, int M, int N, int K, const void* x, int ldx, cons
  * lora_A: [t_cols, K] with t_cols = 64 (one target, rank zero-padded to 64) or 192 (stacked q|k|v A
  * factors, RF_EPI_QKV); lora_B: [N, 64] (rank zero-padded).  M >= 128, N % 128 == 0, K % 64 == 0;
  * epilogues GELU / GATE_RES / QKV.  workspace: rf_op_linear_lora_workspace_bytes(M) bytes of device
- * memory, zero-initialised once by the caller (split-K partials, the bf16 down-projection and the
- * reduction counters live there).  The down-projection runs as one chip-filling split-K launch; the
- * environment switch RF_LORA_DOWN=side selects the four-CTA full-K kernel that rf_dit_forward /
- * rf_dit_denoise fork under their main GEMM (same result up to the fp32 summation order). */
+ * memory (the bf16 down-projection lives there).  The down-projection runs as one GEMM launch with one
+ * CTA per 128 x 64-column output tile (8-32 CTAs at M = 1024), full K per tile; the environment switch
+ * RF_LORA_DOWN=side caps it at the four CTAs that rf_dit_forward / rf_dit_denoise fork onto a second
+ * stream (same result). */
 size_t rf_op_linear_lora_workspace_bytes(int M);
 int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx, const void* W,
                       const void* bias, void* y, int ldy, const void* lora_A, int t_cols,

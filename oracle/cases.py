@@ -1,10 +1,12 @@
 """Seeded parity cases shared by oracle/make_golden.py (reference vs oracle, build container) and
-tests/ (oracle vs golden on CPU; CUDA path vs oracle/golden on the B200).  TEST INFRASTRUCTURE.
+tests/ (oracle vs golden on CPU; CUDA path vs oracle/golden on the GPU).  TEST INFRASTRUCTURE.
 
 Every tensor is a pure function of (case name, seed): nothing but the expected outputs needs to
 be stored in tests/golden/."""
 from __future__ import annotations
 
+import os
+import zlib
 from dataclasses import dataclass, field
 from typing import Dict, Optional
 
@@ -148,3 +150,25 @@ def run_oracle(case: Case, dtype=torch.bfloat16, model=None, lora=None):
     return fo.transformer_forward(model, x["latents"], x["prompt_embeds"], x["pooled"],
                                   x["timestep"], x["img_ids"], x["txt_ids"], x["guidance"],
                                   x["cond_latents"], x["cond_ids"], mc, ls)
+
+
+# ---- stored golden outputs: a seeded sample of GOLDEN_ROWS token rows per case keeps the file small; every
+# comparison against the golden runs on the same rows (`golden_sample`)
+GOLDEN_ROWS = 64
+GOLDEN_FILE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                           "flux_golden.safetensors")
+
+
+def golden_rows(name: str, n_tok: int) -> torch.Tensor:
+    g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+    return torch.randperm(n_tok, generator=g)[:min(GOLDEN_ROWS, n_tok)].sort().values
+
+
+def golden_sample(gold: Dict[str, torch.Tensor], name: str, t: torch.Tensor) -> torch.Tensor:
+    """the golden rows of case `name` of an output [batch, n_tok, 64]"""
+    return t[:, gold[name + "/rows"]]
+
+
+def load_golden() -> Dict[str, torch.Tensor]:
+    from safetensors.torch import load_file
+    return load_file(GOLDEN_FILE)

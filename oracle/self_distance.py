@@ -22,9 +22,8 @@ CASES = ["fwdA_small", "fwdB_small", "fwdA_deep", "fwdB_1024", "denoiseA_28", "d
 
 
 def main():
-    from safetensors.torch import load_file
     ns = ref_loader.load()
-    gold = load_file(os.path.join(REPO, "tests", "golden", "flux_golden.safetensors"))
+    gold = C.load_golden()
     out = {}
     for name in CASES:
         case = C.CASES[name]
@@ -33,7 +32,7 @@ def main():
                                      ("t8_nomkldnn", os.cpu_count() or 8, False)):
             torch.set_num_threads(threads)
             with torch.backends.mkldnn.flags(enabled=mkldnn):
-                runs[tag] = make_golden.run_reference(ns, case).float()
+                runs[tag] = C.golden_sample(gold, name, make_golden.run_reference(ns, case).float())
         torch.set_num_threads(os.cpu_count() or 8)
         true32 = gold[name + "/fp32"].float()
         base = runs["t8"]

@@ -11,7 +11,7 @@ import os
 from ctypes import c_char_p, c_float, c_int, c_int64, c_void_p, POINTER
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# RF_B200_LIB: load another build of the same library (kernel A/B experiments, tools/attn_ab.py)
+# RF_B200_LIB: load another build of the same library (kernel A/B experiments across builds)
 LIB_PATH = os.environ.get("RF_B200_LIB") or os.path.join(_HERE, "librf_b200.so")
 
 _lib = None
@@ -103,7 +103,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise RFError(
                 f"{LIB_PATH} not found: build it with `python __graft_entry__.py build` "
-                "(nvcc, sm_100a). There is no CPU or PyTorch fallback for the DiT hot path.")
+                "(nvcc, sm_90a). There is no CPU or PyTorch fallback for the DiT hot path.")
         lib = ctypes.CDLL(LIB_PATH)
         _declare(lib)
         _lib = lib

@@ -1,5 +1,5 @@
 // dit.cu — host orchestration of the FLUX.1-dev DiT forward and denoise loop (C ABI:
-// rf_dit_* in include/rf_b200.h) over the sm_100a kernels of this directory.
+// rf_dit_* in include/rf_b200.h) over the sm_90a kernels of this directory.
 //
 // Mirrors, launch by launch, what the reference executes per step:
 //   train_flux/flux/transformer.py:47-252 (tranformer_forward; with n_cond == 0 the stock
@@ -34,7 +34,6 @@ int select_row_launch(const bf16* table, int64_t row_elems, const int* row, bf16
                       cudaStream_t stream);
 int f32_to_bf16_launch(const float* src, bf16* dst, int n, cudaStream_t stream);
 int gemm_init();
-int lora_down_init();
 int attention_init();
 int gemv_init();
 }
@@ -113,7 +112,6 @@ struct rf_dit {
   // ---- workspace
   bf16 *X = nullptr, *XN = nullptr, *QKV = nullptr, *ACT = nullptr, *MOD = nullptr, *MODC = nullptr;
   bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [rows, 192], L [rows, 4D]
-  void* lora_ws = nullptr;            // split-K workspace of the LoRA down-projection
   bf16 *emb_tmp = nullptr;            // small vectors for the temb path
   bf16 *temb = nullptr, *ctemb = nullptr;
   // ---- staging for the graph-captured denoise loop
@@ -129,7 +127,7 @@ struct rf_dit {
   cudaStream_t own_stream = nullptr;  // capture is illegal on the legacy default stream
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   int64_t graph_kernels = 0;  // kernel launches inside one captured step
-  // forked stream of the LoRA down-projections: they run on two reserved TPCs UNDER the other token streams'
+  // forked stream of the LoRA down-projections: they run on a few reserved SMs beside the other token streams'
   // GEMM of the same layer (lora_down_side_launch) and join before the condition stream's launch
   cudaStream_t side_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -534,11 +532,11 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     if (rf::gemm2_lora_eligible(epi, N, K, gc)) {
       const bf16* T = t_pre;
       if (T == nullptr && ngr > 1 && side_lora) {
-        // fork: the down-projection runs on kLdSideClusters reserved TPCs while the other streams' GEMM has the rest
+        // fork: the down-projection runs on kLoraSideCtas reserved SMs while the other streams' GEMM has the rest
         RF_CHECK_CUDA(cudaEventRecord(h->ev_fork, s));
-        const int prev = rf::gemm2_reserve_pairs(rf::kLdSideClusters);
+        const int prev = rf::gemm_reserve_sms(rf::kLoraSideCtas);
         const int mrc = rf::gemm_launch(epi, N, K, ngr - 1, gr, s);
-        rf::gemm2_reserve_pairs(prev);
+        rf::gemm_reserve_sms(prev);
         if (mrc) return mrc;
         RF_CHECK_CUDA(cudaStreamWaitEvent(h->side_stream, h->ev_fork, 0));
         RF_TRY(rf::lora_down_side_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, h->side_stream));
@@ -547,7 +545,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
         return rf::gemm2_lora_launch(epi, N, K, gc, h->LT, t_cols, loraB, sec_cols, s);
       }
       if (T == nullptr) {
-        RF_TRY(rf::lora_down_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, h->lora_ws, s));
+        RF_TRY(rf::lora_down_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, s));
         T = h->LT;
         ld_t = t_cols;
       }
@@ -730,8 +728,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     // (forked form: the launch of T happens inside gemm_cond_lora, with all 4 x 64 columns)
     const bool t4_side = t4 && side_lora && ng > 1;
     if (t4 && !t4_side)
-      RF_TRY(rf::lora_down_launch(g[ng - 1].A, D, S_cond.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad,
-                                  h->lora_ws, s));
+      RF_TRY(rf::lora_down_launch(g[ng - 1].A, D, S_cond.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad, s));
     if (cond_lora) {
       RF_TRY(gemm_cond_lora(rf::EPI_QKV, D3, D, ng, g, b.qkvA, t4_side ? 4 * kLoraPad : 3 * kLoraPad, b.qkvB, D,
                             [&](rf::GemmGroupArgs& gc) {
@@ -935,7 +932,7 @@ int rf_dit_create(const rf_dit_config* cfg, rf_dit** out) {
   }
   cudaGetDevice(&h->device);
   // opt in to the large dynamic shared-memory carve-outs up front (not inside a graph capture)
-  if (rf::gemm_init() || rf::lora_down_init() || rf::attention_init() || rf::gemv_init()) {
+  if (rf::gemm_init() || rf::attention_init() || rf::gemv_init()) {
     delete h;
     return -2;
   }
@@ -1106,12 +1103,6 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     const size_t lrows = static_cast<size_t>(std::max(n_cond, 1));
     if (!(p = A(std::max(lrows * 4 * kLoraPad * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LT = static_cast<bf16*>(p);
     if (!(p = A(std::max(lrows * 4 * D * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LL = static_cast<bf16*>(p);
-    {
-      const size_t wsb = rf::lora_down_workspace_bytes(std::max(n_cond, 1), 4 * kLoraPad);
-      if (!(p = A(wsb))) return -2;
-      h->lora_ws = p;
-      RF_CHECK_CUDA(cudaMemsetAsync(p, 0, wsb, s));
-    }
     if (!(p = A(static_cast<size_t>(512 + 4 * D) * 2))) return -2; h->emb_tmp = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->temb = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->ctemb = static_cast<bf16*>(p);

@@ -1,4 +1,4 @@
-// elementwise.cu — the HBM-bound kernels of the DiT step (sm_100a).
+// elementwise.cu — the HBM-bound kernels of the DiT step (sm_90a).
 //
 //   ln_modulate   : LayerNorm(no affine, eps 1e-6) + adaLN scale/shift in one pass over the
 //                   hidden state; writes the bf16 A operand of the next GEMM.
@@ -56,15 +56,14 @@ ln_modulate_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ out, 
 #pragma unroll
   for (int i = 0; i < kLnMaxChunks; ++i)
     if (i < nch) raw[i] = __ldg(xr + lane + 32 * i);
-  // two elements per instruction (FADD2 / FFMA2 / FMUL2, IEEE round-to-nearest like the scalar forms): the
-  // first version issued ~20 scalar instructions per element and ran at 0.33 IPC per scheduler
+  // element pairs (IEEE round-to-nearest like the scalar forms), unpacked from bf16x2 once
   float2 s2 = make_float2(0.f, 0.f);
 #pragma unroll
   for (int i = 0; i < kLnMaxChunks; ++i) {
     if (i < nch) {
       const uint32_t w[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
 #pragma unroll
-      for (int q = 0; q < 4; ++q) s2 = __fadd2_rn(s2, unpack_bf16x2(w[q]));
+      for (int q = 0; q < 4; ++q) s2 = fadd2(s2, unpack_bf16x2(w[q]));
     }
   }
   const float mean = warp_sum(s2.x + s2.y) / static_cast<float>(dim);
@@ -76,8 +75,8 @@ ln_modulate_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ out, 
       const uint32_t w[4] = {raw[i].x, raw[i].y, raw[i].z, raw[i].w};
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float2 d = __fadd2_rn(unpack_bf16x2(w[q]), nmean);
-        q2 = __ffma2_rn(d, d, q2);
+        const float2 d = fadd2(unpack_bf16x2(w[q]), nmean);
+        q2 = ffma2(d, d, q2);
       }
     }
   }
@@ -95,13 +94,13 @@ ln_modulate_kernel(const bf16* __restrict__ x, int ldx, bf16* __restrict__ out, 
       uint32_t ou[4];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        float2 y = __fmul2_rn(__fadd2_rn(unpack_bf16x2(w[q]), nmean), rstd2);   // LayerNorm
+        float2 y = fmul2(fadd2(unpack_bf16x2(w[q]), nmean), rstd2);   // LayerNorm
         bf16_round2(y.x, y.y);                                                      //   -> bf16
-        float2 t = __fadd2_rn(unpack_bf16x2(su[q]), make_float2(1.0f, 1.0f));      // (1 + scale)
+        float2 t = fadd2(unpack_bf16x2(su[q]), make_float2(1.0f, 1.0f));      // (1 + scale)
         bf16_round2(t.x, t.y);                                                      //   -> bf16
-        y = __fmul2_rn(y, t);
+        y = fmul2(y, t);
         bf16_round2(y.x, y.y);                                                      //   -> bf16
-        const float2 o = __fadd2_rn(y, unpack_bf16x2(hu[q]));                      // + shift -> bf16 at the pack
+        const float2 o = fadd2(y, unpack_bf16x2(hu[q]));                      // + shift -> bf16 at the pack
         ou[q] = pack_bf16x2(o.x, o.y);
       }
       orow[lane + 32 * i] = make_uint4(ou[0], ou[1], ou[2], ou[3]);
@@ -124,7 +123,7 @@ static int ln_launch_common(const bf16* x, int ldx, bf16* out, int ldo, int rows
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   int blocks = (rows + 7) / 8;
   if (blocks > sms * 3) blocks = sms * 3;
@@ -244,7 +243,7 @@ static int gemv_launch_nb(const bf16* x, int ldx, const bf16* W, const bf16* bia
   const size_t smem = static_cast<size_t>(NB) * K * sizeof(float);
   if (int rc = gemv_set_attr<NB>()) return rc;
   int blocks = (N + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   ProfScope prof("gemv", 2.0 * NB * N * K, 2.0 * N * K, stream);
   RF_CHECK_CUDA(launch_pdl(gemv_kernel<NB>, dim3(blocks), dim3(256), smem, stream, x, ldx, W, bias, y, ldy, N, K, act));
   count_launch();

@@ -10,9 +10,7 @@
 
 namespace rf {
 bool pdl_enabled() {
-  // opt-in (RF_PDL=1): measured on B200 inside the captured step graph it is within run-to-run noise
-  // (entry A 63.65 vs 63.88 ms, entry B 96.2 vs 94.1 ms; profiles/r02_summary.md), so the default stays
-  // plain stream order
+  // opt-in (RF_PDL=1): the default is plain stream order
   static const bool on = getenv("RF_PDL") && getenv("RF_PDL")[0] == '1';
   return on;
 }
@@ -54,14 +52,12 @@ int resize_u8_launch(const uint8_t* in, int H, int W, uint8_t* tmp, uint8_t* out
                      const int* bx, const int* kx, int ksx, const int* by, const int* ky, int ksy,
                      cudaStream_t stream);
 }
-namespace rf { void dbg_set_attn_trace(long long* p); void dbg_set_gemm_trace(long long* p); void dbg_force_gemm_v1(bool on); }
+namespace rf { void dbg_force_gemm_v1(bool on); }
 
 extern "C" {
 
-// dev-only: timeline buffer (24 x 16 int64, device) for CTA 0 of the next attention launches
+// test hook: 1 = the next GEMM launches use tiles at most 128 wide (covers both tile widths at small shapes)
 void rf_dbg_force_gemm_v1(int on) { rf::dbg_force_gemm_v1(on != 0); }
-void rf_dbg_set_gemm_trace(void* dev_buf) { rf::dbg_set_gemm_trace(static_cast<long long*>(dev_buf)); }
-void rf_dbg_set_attn_trace(void* dev_buf) { rf::dbg_set_attn_trace(static_cast<long long*>(dev_buf)); }
 
 
 const char* rf_last_error(void) { return rf::get_error(); }
@@ -139,7 +135,7 @@ int rf_op_linear(int epilogue, int M, int N, int K, const void* x, int ldx, cons
 
 size_t rf_op_linear_lora_workspace_bytes(int M) {
   const size_t rows = (static_cast<size_t>(M > 0 ? M : 1) + 127) / 128 * 128;
-  return ((rf::lora_down_workspace_bytes(M > 0 ? M : 1, 192) + 255) / 256) * 256 + rows * 192 * 2 + 256;
+  return rows * 192 * 2 + 256;
 }
 
 int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx, const void* W,
@@ -172,14 +168,13 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
     return -1;
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // workspace = [split-K partials + counters | T (bf16 [rows, t_cols])]
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  bf16* T = reinterpret_cast<bf16*>(ws + ((rf::lora_down_workspace_bytes(M, 192) + 255) / 256) * 256);
-  // RF_LORA_DOWN=side: the confined few-CTA form the DiT forks under its main GEMM (here on the caller's stream)
+  // workspace = T (bf16 [rows, t_cols])
+  bf16* T = static_cast<bf16*>(workspace);
+  // RF_LORA_DOWN=side: the confined few-CTA form the DiT forks beside its main GEMM (here on the caller's stream)
   const char* form = getenv("RF_LORA_DOWN");
   int rc = (form && strcmp(form, "side") == 0)
                ? rf::lora_down_side_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, s)
-               : rf::lora_down_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, ws, s);
+               : rf::lora_down_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, s);
   if (rc) return rc;
   return rf::gemm2_lora_launch(epilogue, N, K, g, T, t_cols, static_cast<const bf16*>(lora_B),
                                t_cols == 192 ? N / 3 : 0, s);

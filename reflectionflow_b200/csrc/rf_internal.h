@@ -94,7 +94,7 @@ struct GemmGroupArgs {
 int gemm_launch(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups,
                 cudaStream_t stream);
 
-// One token stream with peft's unfused LoRA arithmetic fused into the GEMM (gemm2cta_sm100.cu):
+// One token stream with peft's unfused LoRA arithmetic fused into the GEMM (gemm_sm90.cu, kLora):
 //   out = epi( bf16( bf16(A W^T + b) + bf16(T loraB^T) ) ),  T = bf16(A loraA^T) computed beforehand.
 // T: [M, ldT]; with sec_cols > 0 output section s = n / sec_cols reads T columns [64 s, 64 s + 64)
 // (stacked q|k|v); loraB: [N, 64] (rank zero-padded to 64).
@@ -102,24 +102,22 @@ bool gemm2_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a);
 int gemm2_lora_launch(int epi, int N, int K, const GemmGroupArgs& a, const bf16* T, int ldT,
                       const bf16* loraB, int sec_cols, cudaStream_t stream);
 
-// LoRA down-projection of one token stream: T[M, NT] = bf16(X[M, K] @ A[NT, K]^T), NT = 64 | 192 | 256,
-// split-K over the SMs with a deterministic in-kernel reduction (lora_down_sm100.cu).  `ws` holds
-// lora_down_workspace_bytes(M, NT) bytes and must be zeroed once before its first use.
-size_t lora_down_workspace_bytes(int M, int NT);
+// LoRA down-projection of one token stream: T[M, NT] = bf16(X[M, K] @ A[NT, K]^T), NT a multiple of 64,
+// on the GEMM kernel above (fp32 accumulation over the whole K, one rounding).
 int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
-                     void* ws, cudaStream_t stream);
-// The same product on kLdSideClusters TPCs only (2-CTA clusters walking full-K items), for a forked stream that
-// runs under a CTA-pair GEMM launched with gemm2_reserve_pairs(kLdSideClusters).  NT: any multiple of 64.
-static constexpr int kLdSideClusters = 2;
+                     cudaStream_t stream);
+// The same product on kLoraSideCtas SMs only, for a forked stream that runs beside a GEMM launched with
+// gemm_reserve_sms(kLoraSideCtas).
+static constexpr int kLoraSideCtas = 4;
 int lora_down_side_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
                           cudaStream_t stream);
-// The next CTA-pair GEMM launches of this thread leave `pairs` TPCs free when that does not add a wave of tiles
-// (0 = use every TPC).  Returns the previous value.
-int gemm2_reserve_pairs(int pairs);
+// The next GEMM launches of this thread leave `sms` SMs free when that does not add a wave of tiles
+// (0 = use every SM).  Returns the previous value.
+int gemm_reserve_sms(int sms);
 
 // ---------------------------------------------------------------------------- attention
 // Non-causal softmax(Q K^T / sqrt(128)) V over one joint token sequence.
-// qkv: [n_tok, ld_qkv] with q at column 0, k at +q_stride... (see attn_sm100.cu)
+// q, k, v: token-major [n_tok, heads*128] slices of one buffer (see attn_sm90.cu)
 struct AttnArgs {
   const bf16* q; const bf16* k; const bf16* v;  // each [n_tok, heads*128] slices, pitch ld_qkv
   int ld_qkv;
@@ -131,7 +129,7 @@ struct AttnArgs {
 };
 int attention_launch(const AttnArgs& a, cudaStream_t stream);
 
-// T5 / CLIP self-attention, head_dim 64, S <= 512, on tcgen05 (text_attn_sm100.cu): eager-attention
+// T5 / CLIP self-attention, head_dim 64, S <= 512, on wgmma (text_attn_sm90.cu): eager-attention
 // rounding points (scores -> bf16 [* scale -> bf16] [+ bias -> bf16], fp32 softmax -> bf16, PV -> bf16)
 bool text_attn_tc_eligible(int S, int ld, int ldo);
 int text_attn_tc_launch(const bf16* q, const bf16* k, const bf16* v, int ld, bf16* out, int ldo, int B, int S,

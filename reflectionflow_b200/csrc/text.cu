@@ -1,4 +1,4 @@
-// text.cu — T5 encoder (T5-v1.1-XXL shape) and CLIP text encoder on sm_100a, behind rf_text_* (C ABI).
+// text.cu — T5 encoder (T5-v1.1-XXL shape) and CLIP text encoder on sm_90a, behind rf_text_* (C ABI).
 //
 // Replaces `pipe.text_encoder_2(ids)[0]` (T5, prompt_embeds [B, 512, 4096]) and
 // `pipe.text_encoder(ids).pooler_output` (CLIP-L, pooled [B, 768]) inside diffusers
@@ -6,7 +6,7 @@
 // pipeline_tools.py:33-52) — each reflection candidate has its own refined prompt
 // (tts/tts_reflectionflow.py:286-294).  Token ids in (tokenizers stay on the host), embeddings out.
 //
-// All Linear layers run on the tcgen05 GEMM kernels of this library (fused residual / GELU
+// All Linear layers run on the wgmma GEMM kernel of this library (fused residual / GELU
 // epilogues); the pieces specific to the text encoders are small bandwidth kernels here: T5 RMSNorm,
 // affine LayerNorm, embedding gathers, the gated-GELU product, quick-GELU, and a shared-memory
 // attention for short sequences with head_dim 64 (T5: additive relative-position bias, no scaling;
@@ -350,7 +350,7 @@ int linear(int epi, const bf16* A, int lda, int M, const bf16* W, const bf16* bi
 }
 int small_attn(const bf16* q, const bf16* k, const bf16* v, int ld, bf16* out, int ldo, int B, int S, int heads,
                const bf16* bias, float scale, int use_scale, int causal, cudaStream_t s) {
-  // tensor-core path (text_attn_sm100.cu); RF_TEXT_ATTN=smem keeps the CUDA-core kernel below for A/B runs
+  // tensor-core path (text_attn_sm90.cu); RF_TEXT_ATTN=smem keeps the CUDA-core kernel below for A/B runs
   static const bool force_smem = getenv("RF_TEXT_ATTN") && std::string(getenv("RF_TEXT_ATTN")) == "smem";
   if (!force_smem && rf::text_attn_tc_eligible(S, ld, ldo))
     return rf::text_attn_tc_launch(q, k, v, ld, out, ldo, B, S, heads, bias, scale, use_scale, causal, s);

@@ -1,4 +1,4 @@
-// vae.cu — FLUX VAE decoder (diffusers AutoencoderKL.decode) on sm_100a, behind rf_vae_* (C ABI).
+// vae.cu — FLUX VAE decoder (diffusers AutoencoderKL.decode) on sm_90a, behind rf_vae_* (C ABI).
 //
 // Replaces `vae.decode(latents / scaling + shift)` + `image_processor.postprocess` at
 // train_flux/flux/generate.py:302-307 (and diffusers FluxPipeline.__call__'s tail): packed latents
@@ -6,7 +6,7 @@
 //
 // Layout: activations are NHWC bf16 with a one-pixel zero ring, flattened to [(H+2)(W+2), C], so a
 // 3x3 convolution is an implicit GEMM whose A tile for tap (dy, dx) is just a row-shifted TMA box
-// of the same tensor (gemm2cta_sm100.cu, conv mode: tcgen05 cta_group::2, bias / residual fused in
+// of the same tensor (gemm_sm90.cu, conv mode: wgmma, bias / residual fused in
 // the epilogue).  GroupNorm(32)+SiLU, nearest 2x upsampling, the latent unpack and the uint8
 // post-process are bandwidth kernels here.  The mid-block self-attention (16384 tokens, one head of
 // 512) runs as QK^T GEMM -> row softmax -> PV GEMM on the same GEMM kernel.
@@ -61,7 +61,7 @@ __global__ void unpack_latents_kernel(const bf16* __restrict__ packed, bf16* __r
 // Deterministic (no atomics): fixed-order reduction inside the block, one partial row per block,
 // partial rows summed in block order by the finalize kernel — a run-to-run difference in the last
 // bit of a mean could flip a bf16 rounding downstream and with it a candidate's score.
-static constexpr int kGnBlocks = 148 * 4;
+static constexpr int kGnBlocks = 132 * 4;
 __global__ void __launch_bounds__(256)
 gn_stats_kernel(const bf16* __restrict__ x, int H, int W, int C, int padded, float* __restrict__ part) {
   __shared__ float sm[256][4];
@@ -485,7 +485,7 @@ size_t padded_elems(int H, int W, int C) { return static_cast<size_t>(H + 2) * (
 
 int grid_for(long long work, int threads = 256) {
   long long b = (work + threads - 1) / threads;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   return static_cast<int>(b < 1 ? 1 : b);
 }
 
@@ -505,8 +505,8 @@ int group_norm(rf_vae* h, const bf16* x, bf16* out, int H, int W, const Norm& n,
   {
     rf::ProfScope prof("vae_gn_apply", 0, 4.0 * H * W * C, s);
     // rows x row slices: ~16 CTAs per SM in flight, every thread >= 1 vector of its row slice
-    const int rows = H < 148 * 16 ? H : 148 * 16;
-    int slices = (148 * 16 + rows - 1) / rows;
+    const int rows = H < 132 * 16 ? H : 132 * 16;
+    int slices = (132 * 16 + rows - 1) / rows;
     const int max_slices = (W * (C / 8) + 255) / 256;
     if (slices > max_slices) slices = max_slices;
     rf::gn_apply_kernel<<<dim3(rows, slices), 256, 0, s>>>(

@@ -7,7 +7,7 @@
   entry B  `tranformer_forward(transformer, condition_latents, condition_ids, condition_type_ids,
             model_config, c_t, **params)`  — train_flux/flux/transformer.py:47-55
 
-Both run the same C-ABI call (rf_dit_forward, include/rf_b200.h) on hand-written sm_100a
+Both run the same C-ABI call (rf_dit_forward, include/rf_b200.h) on hand-written sm_90a
 kernels.  There is no PyTorch fallback: without librf_b200.so or without a GPU this raises.
 """
 from __future__ import annotations

@@ -6,7 +6,7 @@ take the top-k indices (:123-124), then let the refiner rewrite every current pr
 evaluation, original prompt, current prompt) for the next round (:127-137); `refined_prompt<r>` is appended
 to `best_img_meta.jsonl` (:139-140).
 
-B200 form: the candidates of a round are sharded over the ranks (one process per GPU), final latents and
+Sharded form: the candidates of a round are sharded over the ranks (one process per GPU), final latents and
 score records are all-gathered (as in `reflectionflow.sample`), every rank derives the same ranking, the LLM
 hook runs on rank 0 and its text is broadcast.  The verifier / refiner networks are external models behind
 `verifiers.load_verifier` / the reflector classes (stubs offline)."""

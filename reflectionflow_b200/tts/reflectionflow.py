@@ -1,4 +1,4 @@
-"""ReflectionFlow search loop on B200s — mirror of tts/tts_reflectionflow.py (sample :94-463,
+"""ReflectionFlow search loop on sharded GPUs — mirror of tts/tts_reflectionflow.py (sample :94-463,
 main :466-629): per round  score parents -> top-k -> reflect -> refine prompt -> regenerate each
 candidate conditioned on its parent -> re-score -> chain bookkeeping.
 

@@ -1,6 +1,6 @@
 """Selection, bookkeeping and sharding logic of the outer loop — pure functions so that they can be
 pinned by table tests (reference: tts/tts_reflectionflow.py:144-182,359-448) — plus the one
-collective the B200 design adds: an all-gather of fixed-size score records per round
+collective the sharded design adds: an all-gather of fixed-size score records per round
 (SURVEY.md §8e)."""
 from __future__ import annotations
 

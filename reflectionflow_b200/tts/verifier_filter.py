@@ -4,7 +4,7 @@ are listed round by round (rounds in numeric order, files of a round in name ord
 prompt with the NVILA-shaped verifier (:107-113), and for N in 1, 2, 4, 8, 16, 32 the best of the FIRST N
 candidates under the yes/no sort key (:119-123) is copied to `NNNNN/nfe<N>/00000.png` (:126-173).
 
-B200 form: scoring is sharded over the ranks and exchanged as fixed-size records (same helpers as the search
+Sharded form: scoring is sharded over the ranks and exchanged as fixed-size records (same helpers as the search
 loops); every rank derives the same choices, rank 0 writes the files.  Candidates stored as `*.latent.pt`
 (this framework always writes the packed latent next to the PNG) can be scored without a decode by verifiers
 that do not need pixels, and are decoded through `pipe.vae` for the ones that do."""

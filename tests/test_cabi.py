@@ -26,17 +26,19 @@ def test_library_exports_every_declared_symbol():
     assert lib.rf_abi_version() == 2
 
 
-def test_sass_is_blackwell_native():
-    """tcgen05 / TMA / TMEM instructions are present in the shipped binary (B200_PROFILING.md)."""
+def test_sass_is_hopper_native():
+    """the shipped binary is sm_90a code whose tensor-core work is wgmma (HGMMA) fed by TMA (UTMALDG)."""
     import shutil
     import subprocess
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not on PATH")
     so = os.path.join(ROOT, "reflectionflow_b200", "librf_b200.so")
     sass = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "UTMALDG", "LDTM", "STTM"):
+    archs = set(re.findall(r"arch = (sm_\w+)", sass))
+    assert archs == {"sm_90a"}, archs
+    for mnem in ("HGMMA.", "UTMALDG", "SYNCS."):
         assert mnem in sass, mnem
-    assert "HMMA." not in sass.replace("UTCHMMA", ""), "legacy mma.sync path must not be present"
+    assert "HMMA." not in sass.replace("HGMMA.", ""), "legacy mma.sync path must not be present"
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

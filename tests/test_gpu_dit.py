@@ -29,8 +29,7 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def _golden():
-    from safetensors.torch import load_file
-    return load_file(os.path.join(GOLD, "flux_golden.safetensors")), json.load(
+    return C.load_golden(), json.load(
         open(os.path.join(GOLD, "flux_golden.json")))
 
 
@@ -77,7 +76,9 @@ def test_dit_matches_reference_golden(name):
     gold, meta = _golden()
     ref_bf16 = gold[name + "/bf16"].float()
     true32 = gold[name + "/fp32"].float()
-    ours = _run_cuda(case).float()
+    full = _run_cuda(case).float()
+    assert torch.isfinite(full).all()
+    ours = C.golden_sample(gold, name, full)  # the stored rows of the case
     assert ours.shape == ref_bf16.shape
     assert torch.isfinite(ours).all()
     e_ours = (ours - true32).abs()
@@ -104,7 +105,7 @@ def test_merged_lora_mode_stays_inside_the_error_budget(name):
     _, lora = C.build_model(case)
     m.load_lora(lora, mode="merged")
     try:
-        ours = _run_cuda(case).float()
+        ours = C.golden_sample(gold, name, _run_cuda(case).float())
     finally:
         m.load_lora(lora, mode="exact")
     true32, ref = gold[name + "/fp32"].float(), gold[name + "/bf16"].float()
@@ -129,7 +130,7 @@ def test_entry_a_forward_surface_and_determinism():
     torch.cuda.synchronize()
     assert torch.equal(a, b)
     gold, _ = _golden()
-    d = (a.cpu().float() - gold["fwdA_small/bf16"].float()).abs()
+    d = (C.golden_sample(gold, "fwdA_small", a.cpu().float()) - gold["fwdA_small/bf16"].float()).abs()
     assert d.mean() < 0.05
 
 
@@ -227,11 +228,11 @@ def test_k_only_adapter_is_applied():
 
 @pytest.mark.parametrize("name", ["fwdB_1024", "denoiseB_1024_28", "fwdB_full_c256"])
 def test_forked_schedule_is_deterministic_and_equivalent(name, monkeypatch):
-    """The step forks work onto a second stream (csrc/dit.cu): the LoRA down-projections run on two reserved TPCs
-    under the image + text GEMM of the same layer.  The forked schedule must be bit-reproducible run to run (eager
+    """The step forks work onto a second stream (csrc/dit.cu): the LoRA down-projections run on a few reserved SMs
+    beside the image + text GEMM of the same layer.  The forked schedule must be bit-reproducible run to run (eager
     forward and captured graph) and must agree with the single-stream schedule up to the one legitimate difference:
-    the confined down-projection accumulates the whole K in one CTA, the single-stream one sums split-K partials (fp32
-    summation order, then the same bf16 rounding; a 28-step loop amplifies the few 1-ulp flips of T).  Both schedules
+    any difference in fp32 summation order of the down-projection, then the same bf16 rounding (a 28-step loop
+    amplifies the few 1-ulp flips of T).  Both schedules
     must meet the error budget against the fp32 evaluation on their own.  The switch is read at enqueue / capture time."""
     case = C.CASES[name]
     m = _build(case)
@@ -245,6 +246,7 @@ def test_forked_schedule_is_deterministic_and_equivalent(name, monkeypatch):
     assert torch.isfinite(a).all() and torch.isfinite(b).all()
     assert torch.equal(outs["forked"], outs["forked-again"])
     gold, _ = _golden()
+    a, b = C.golden_sample(gold, name, a), C.golden_sample(gold, name, b)
     true32 = gold[name + "/fp32"].float()
     e_ref = (gold[name + "/bf16"].float() - true32).abs().mean()
     d = (a - b).abs().mean()
@@ -263,13 +265,14 @@ def test_fused_lora_term_is_really_applied(name):
     the CUDA output must be far closer to the reference WITH the adapter than to the oracle WITHOUT it."""
     case = C.CASES[name]
     gold, _ = _golden()
-    ours = _run_cuda(case).float()
+    ours = C.golden_sample(gold, name, _run_cuda(case).float())
     with_lora = gold[name + "/bf16"].float()
     model, _ = C.build_model(case)
     x = C.build_inputs(case)
     no_lora = fo.transformer_forward(model, x["latents"], x["prompt_embeds"], x["pooled"], x["timestep"],
                                      x["img_ids"], x["txt_ids"], x["guidance"], x["cond_latents"], x["cond_ids"],
                                      C.oracle_model_config(case), None).float()
+    no_lora = C.golden_sample(gold, name, no_lora)
     d_with, d_without, effect = (ours - with_lora).abs().mean(), (ours - no_lora).abs().mean(), (with_lora - no_lora).abs().mean()
     print(f"[{name}] |ours - ref(with LoRA)| {d_with:.4g} ; |ours - oracle(no LoRA)| {d_without:.4g} ; adapter effect {effect:.4g}")
     assert effect > 2e-3, "the adapter must matter for this test to mean anything"

@@ -1,4 +1,4 @@
-"""-m gpu: operator-level parity of the sm_100a kernels, called through the C ABI (ctypes), against
+"""-m gpu: operator-level parity of the sm_90a kernels, called through the C ABI (ctypes), against
 plain torch fp32 restatements of the same op with the reference's bf16 rounding points
 (SURVEY.md Appendix A).  Tolerances are stated per test."""
 import math
@@ -56,8 +56,8 @@ def _call_linear(epi, x, W, bias, y, addend=None, res=None, gate=None, cos=None,
 
 @pytest.fixture(params=["pair", "single"])
 def gemm_path(request):
-    """big shapes run on the CTA-pair kernel (gemm2cta_sm100.cu); `single` forces the 1-CTA kernel
-    (gemm_sm100.cu) so both stay covered"""
+    """big shapes run on 256-wide tiles; `single` forces tiles at most 128 wide so both tile widths of
+    csrc/gemm_sm90.cu stay covered"""
     lib = L.load()
     lib.rf_dbg_force_gemm_v1(1 if request.param == "single" else 0)
     yield request.param
@@ -202,8 +202,8 @@ def _call_linear_lora(epi, x, W, bias, y, Ap, Bp, t_cols, res=None, gate=None, c
 
 @pytest.fixture(params=["split", "side"])
 def lora_down_form(request, monkeypatch):
-    """both forms of T = bf16(x A^T): the split-K launch and the confined few-CTA kernel that the DiT forks under its
-    main GEMM (csrc/lora_down_sm100.cu); the op reads RF_LORA_DOWN at call time"""
+    """both forms of T = bf16(x A^T): the chip-filling launch and the confined few-CTA launch that the DiT forks beside
+    its main GEMM (csrc/gemm_sm90.cu); the op reads RF_LORA_DOWN at call time"""
     monkeypatch.setenv("RF_LORA_DOWN", request.param)
     return request.param
 
@@ -311,7 +311,8 @@ def test_attention(n_tok, heads):
 
 
 def test_attention_sharp_rows():
-    """large score spread exercises the lazy-rescale path (max jumps by > 2^8 between tiles)"""
+    """large score spread: the running row max jumps by > 2^8 between tiles, so the online-softmax rescale of O and the
+    row sums must stay exact"""
     lib = L.load()
     n_tok, heads = 512, 2
     inner = heads * 128

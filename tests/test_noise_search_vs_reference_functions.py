@@ -6,7 +6,7 @@ with `ast` and run over fakes (same method as tests/test_outer_loop_vs_reference
 
 Compared: what the pipeline is called with (prompts per batch, the stacked latents bit for bit, guidance / steps /
 size), the file every image is written to, the returned datapoint, and for the prompt-refinement search the ranking,
-the refined prompts and `best_img_meta.jsonl`.  Needs /root/reference."""
+the refined prompts and `best_img_meta.jsonl`.  What the reference's functions produced is stored under tests/golden/reference/ (tests/_refgold.py)."""
 import ast
 import copy
 import hashlib
@@ -30,9 +30,11 @@ from reflectionflow_b200.tts import noise_scaling as NS  # noqa: E402
 from reflectionflow_b200.tts.dist import DistCtx  # noqa: E402
 from reflectionflow_b200.tts.utils import get_noises  # noqa: E402
 
-REF_NS = "/root/reference/tts/tts_t2i_noise_scaling.py"
-REF_NP = "/root/reference/tts/tts_t2i_noise_prompt_scaling.py"
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_NS), reason="reference tree not present")
+from tests._refgold import Store, norm, ref_path  # noqa: E402
+
+REF_NS = ref_path("tts/tts_t2i_noise_scaling.py")
+REF_NP = ref_path("tts/tts_t2i_noise_prompt_scaling.py")
+GOLD = Store("noise_search")
 
 H = W = 64
 CONFIG = {"pipeline_args": {"height": H, "width": W, "guidance_scale": 3.5, "num_inference_steps": 4},
@@ -86,30 +88,45 @@ class _OurPipe:
         return FluxPipelineOutput(images=(latents.float() * 0.5).to(torch.bfloat16))
 
 
-def _same_calls(a, b):
-    assert len(a) == len(b)
-    for x, y in zip(a, b):
-        assert {k: v for k, v in x.items() if k != "latents"} == {k: v for k, v in y.items() if k != "latents"}
-        assert x["latents"].shape == y["latents"].shape and torch.equal(x["latents"], y["latents"])
+def _calls(calls):
+    """pipeline calls as stored: the latents by shape, dtype and a digest of their bytes"""
+    out = []
+    for c in calls:
+        lat = c["latents"].contiguous()
+        digest = hashlib.sha256(lat.view(torch.uint8).numpy().tobytes() if lat.dtype != torch.bfloat16
+                                else lat.view(torch.int16).numpy().tobytes()).hexdigest()
+        out.append(norm(dict({k: v for k, v in c.items() if k != "latents"},
+                             latents=[list(lat.shape), str(lat.dtype), digest])))
+    return out
+
+
+def _same_calls(stored, ours):
+    assert stored == _calls(ours)
 
 
 def test_noise_scaling_round_equals_the_reference_function(tmp_path):
-    ref_sample = _compile(REF_NS, "sample", dict(torch=torch, DiffusionPipeline=object, copy=copy, os=os))
     torch.manual_seed(8)
     noises = get_noises(2 ** 31 - 1, 5, H, W)
     prompts = [f"a photo of a bench, variant {i}" for i in range(5)]
     mid = str(tmp_path / "samples")
     os.makedirs(mid)
-    rp = _RefPipe()
-    ref_dp = ref_sample(noises, prompts, 3, rp, CONFIG, "a photo of a bench", mid)
+
+    def reference_round():
+        ref_sample = _compile(REF_NS, "sample", dict(torch=torch, DiffusionPipeline=object, copy=copy, os=os))
+        rp = _RefPipe()
+        dp = ref_sample(noises, prompts, 3, rp, CONFIG, "a photo of a bench", str(tmp_path / "ref_samples"))
+        return {"calls": _calls(rp.calls), "saves": [os.path.basename(p) for p in rp.saves], "dp": dp}
+
+    ref = GOLD.value("noise_scaling", reference_round)
     op = _OurPipe()
     our_dp = NS.sample(noises, prompts, 3, op, CONFIG, "a photo of a bench", mid, ctx=DistCtx())
     NS.flush_saves()
-    _same_calls(rp.calls, op.calls)                                  # batches of 2, 2, 1; stacked latents identical
+    _same_calls(ref["calls"], op.calls)                              # batches of 2, 2, 1; stacked latents identical
     assert [c["latents"].shape[0] for c in op.calls] == [2, 2, 1]
-    assert our_dp["generated_img"] == rp.saves                         # <round>_round@<seed>.png, in noise order
-    assert {k: our_dp[k] for k in ref_dp} == ref_dp                    # prompt, search_round, num_noises
-    assert sorted(os.listdir(mid)) == sorted(os.path.basename(p)[:-4] + ".latent.pt" for p in rp.saves)
+    assert [os.path.basename(p) for p in our_dp["generated_img"]] == ref["saves"]  # <round>_round@<seed>.png
+    assert all(os.path.dirname(p) == mid for p in our_dp["generated_img"])
+    assert norm({k: our_dp[k] for k in ref["dp"]}) == ref["dp"]       # prompt, search_round, num_noises
+    assert sorted(os.listdir(mid)) == sorted(p[:-4] + ".latent.pt" for p in ref["saves"])
 
 
 def _verdict(path):
@@ -147,10 +164,6 @@ def test_noise_prompt_scaling_rounds_equal_the_reference_function(tmp_path, seed
         def refine_prompt(self, inputs):
             return [_refined(*item) for item in inputs]
 
-    ref_sample = _compile(REF_NP, "sample", dict(torch=torch, Union=Union, List=List, Optional=Optional,
-                                                  DiffusionPipeline=object, copy=copy, json=json, os=os, time=time,
-                                                  Image=ImageMod, OpenAIVerifier=OpenAIVerifier, verifier=Verifier,
-                                                  yes_id=0, no_id=1))
 
     class OurVerifier:
         needs_images = False
@@ -170,12 +183,18 @@ def test_noise_prompt_scaling_rounds_equal_the_reference_function(tmp_path, seed
     noises = [get_noises(2 ** 31 - 1, branch, H, W) for _ in range(rounds)]
     logs = {}
     cwd = os.getcwd()
-    try:
-        for side in ("ref", "ours"):
-            os.makedirs(tmp_path / side / "run" / "samples")
-            os.chdir(tmp_path / side)
+
+    def run(side):
+        os.makedirs(tmp_path / side / "run" / "samples")
+        os.chdir(tmp_path / side)
+        try:
             prompts, log = ["a green bench"] * branch, []
             pipe = _RefPipe() if side == "ref" else _OurPipe()
+            if side == "ref":
+                ref_sample = _compile(REF_NP, "sample", dict(
+                    torch=torch, Union=Union, List=List, Optional=Optional, DiffusionPipeline=object, copy=copy,
+                    json=json, os=os, time=time, Image=ImageMod, OpenAIVerifier=OpenAIVerifier, verifier=Verifier,
+                    yes_id=0, no_id=1))
             for rnd in range(1, rounds + 1):
                 n0 = len(pipe.calls)
                 if side == "ref":
@@ -186,14 +205,17 @@ def test_noise_prompt_scaling_rounds_equal_the_reference_function(tmp_path, seed
                                    "run/samples", tag="colors", verifier=OurVerifier(), refiner=OurRefiner(),
                                    ctx=DistCtx())
                 prompts = dp["refined_prompt"]
-                log.append({"dp": {k: dp[k] for k in ("original_prompt", "refined_prompt", "search_round",
-                                                      "num_noises", "choice_of_metric")},
-                            "calls": pipe.calls[n0:]})
-            logs[side] = log
-    finally:
-        os.chdir(cwd)
-    for a, b in zip(logs["ref"], logs["ours"]):
+                log.append({"dp": norm({k: dp[k] for k in ("original_prompt", "refined_prompt", "search_round",
+                                                           "num_noises", "choice_of_metric")}),
+                            "calls": _calls(pipe.calls[n0:])})
+        finally:
+            os.chdir(cwd)
+        return {"log": log, "meta": open(tmp_path / side / "run" / "best_img_meta.jsonl").read()}
+
+    ref = GOLD.value(f"noise_prompt_scaling/seed{seed}", lambda: run("ref"))
+    ours = run("ours")
+    assert len(ref["log"]) == len(ours["log"]) == rounds
+    for a, b in zip(ref["log"], ours["log"]):
         assert a["dp"] == b["dp"]
-        _same_calls(a["calls"], b["calls"])
-    assert open(tmp_path / "ref" / "run" / "best_img_meta.jsonl").read() == \
-        open(tmp_path / "ours" / "run" / "best_img_meta.jsonl").read()
+        assert a["calls"] == b["calls"]
+    assert ref["meta"] == ours["meta"]

@@ -323,9 +323,7 @@ def test_main_on_the_reference_config_and_a_reference_written_stage0(tmp_path, m
     `reflectionflow.main`; denoiser and VAE are test-only fakes.  The artefact tree is the one `verifier_filter.py` and
     the GenEval tooling read (tts_reflectionflow.py:562-579, 398-448)."""
     from PIL import Image
-    ref_cfg = "/root/reference/tts/configs/flux.1_dev_nvilascore.json"
-    if not os.path.exists(ref_cfg):
-        pytest.skip("reference tree not present")
+    ref_cfg = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_configs", "flux.1_dev_nvilascore.json")
     stage0 = tmp_path / "stage0" / "00000"
     os.makedirs(stage0 / "samples")
     (stage0 / "metadata.jsonl").write_text(json.dumps({"prompt": "a photo of a kite", "tag": "single_object"}))

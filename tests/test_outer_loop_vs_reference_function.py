@@ -10,7 +10,7 @@ denoiser.  Compared over several rounds with the reference's nvila and gptscore 
 EQUAL grading dicts for different images, where `outputs.index` collapses them, App. B.7): the selected parents, the
 prompt + " [Reflexion]: " + reflection strings and conditions handed to `generate`, the refined prompts / reflections
 carried to the next round, the chains, `best_img_detailedscore.jsonl` and `best_img_meta.jsonl` byte for byte, and
-which candidate lands in samples_lastround / samples_path_bestround / samples_best.  Needs /root/reference."""
+which candidate lands in samples_lastround / samples_path_bestround / samples_best.  What the reference's function produced is stored under tests/golden/reference/ (tests/_refgold.py)."""
 import ast
 import copy
 import hashlib
@@ -34,8 +34,10 @@ from reflectionflow_b200.tts.dist import DistCtx  # noqa: E402
 from reflectionflow_b200.tts.utils import get_noises  # noqa: E402
 from reflectionflow_b200.tts.verifiers import Candidate  # noqa: E402
 
-REF = "/root/reference/tts/tts_reflectionflow.py"
-pytestmark = pytest.mark.skipif(not os.path.exists(REF), reason="reference tree not present")
+from tests._refgold import Store, norm, ref_path  # noqa: E402
+
+REF = ref_path("tts/tts_reflectionflow.py")
+GOLD = Store("outer_loop")
 
 H = W = 64
 COND = 32
@@ -260,20 +262,31 @@ def test_reflection_rounds_equal_the_reference_function(tmp_path, seed, kind, un
     torch.manual_seed(100 + seed)
     noises = [get_noises(2 ** 31 - 1, branch, H, W) for _ in range(rounds)]
     cwd = os.getcwd()
-    try:  # both runs write relative artefact paths under their own directory
+
+    def reference_run():  # the reference's unmodified sample() over the fakes, in its own directory
         os.makedirs(tmp_path / "ref")
         os.chdir(tmp_path / "ref")
-        ref = _run_reference("run", config, rounds, branch, noises, unique)
+        try:
+            log = _run_reference("run", config, rounds, branch, noises, unique)
+        finally:
+            os.chdir(cwd)
+        return {"log": log, "jsonl": {name: open(tmp_path / "ref" / "run" / name).read()
+                                      for name in ("best_img_detailedscore.jsonl", "best_img_meta.jsonl")}}
+
+    stored = GOLD.value(f"{kind}/unique{int(unique)}/seed{seed}", reference_run)
+    try:  # our run writes relative artefact paths under its own directory
         os.makedirs(tmp_path / "ours")
         os.chdir(tmp_path / "ours")
         ours = _run_ours("run", config, rounds, branch, noises, unique)
     finally:
         os.chdir(cwd)
+    ref = stored["log"]
+    assert len(ref) == len(ours) == rounds
     for rnd, (a, b) in enumerate(zip(ref, ours), start=1):
-        assert a["dp"] == b["dp"], f"round {rnd}: datapoint"
-        assert a["chains"] == b["chains"], f"round {rnd}: chains"
+        assert a["dp"] == norm(b["dp"]), f"round {rnd}: datapoint"
+        assert a["chains"] == norm(b["chains"]), f"round {rnd}: chains"
         # the reference generates in batches of batch_size_for_img_gen = 1, in candidate order: same calls
-        assert a["generate"] == b["generate"], f"round {rnd}: what the denoiser was asked for"
+        assert a["generate"] == norm(b["generate"]), f"round {rnd}: what the denoiser was asked for"
         # which candidate was written where (the reference names samples_best with a leaked loop index, App. B.9)
         ref_files = {}
         for dest, src in a["saves"]:
@@ -286,5 +299,5 @@ def test_reflection_rounds_equal_the_reference_function(tmp_path, seed, kind, un
         if rnd > 1:  # files of earlier rounds stay on disk; the reference log holds this round's writes only
             got = {k: v for k, v in got.items() if k in ref_files}
         assert got == ref_files, f"round {rnd}: artefacts"
-    for name in ("best_img_detailedscore.jsonl", "best_img_meta.jsonl"):
-        assert open(tmp_path / "ref" / "run" / name).read() == open(tmp_path / "ours" / "run" / name).read(), name
+    for name, text in stored["jsonl"].items():
+        assert text == open(tmp_path / "ours" / "run" / name).read(), name

@@ -225,7 +225,7 @@ def test_reflection_generator_ours_messages_and_retries(tmp_path):
 
 def test_grading_schemas_equal_the_reference_classes():
     """openai_verifier.py:23-69: every `Grading*` pydantic class of the reference, field for field and in order (read
-    from the reference source when it is present; the pinned table below otherwise)"""
+    from the reference source when recording, tests/_refgold.py; the pinned table below as well)"""
     import ast
     pinned = {None: 6, "single_object": 4, "two_object": 4, "counting": 4, "colors": 4, "position": 4, "color_attr": 4}
     assert {k: len(v) for k, v in V.GRADING_ASPECTS.items()} == pinned
@@ -235,96 +235,131 @@ def test_grading_schemas_equal_the_reference_classes():
         assert model.__name__ == ("Grading" if tag is None else f"Grading_{tag}")
         sub = model.model_fields["overall_score"].annotation
         assert tuple(sub.model_fields) == ("score", "explanation")
-    path = "/root/reference/tts/verifiers/openai_verifier.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present: pinned table only")
-    ref = {}
-    for node in ast.parse(open(path).read()).body:
-        if isinstance(node, ast.ClassDef) and node.name.startswith("Grading"):
-            tag = node.name[len("Grading_"):] or None
-            ref[tag] = tuple(s.target.id for s in node.body if isinstance(s, ast.AnnAssign))
-    assert ref == {k: tuple(v) for k, v in V.GRADING_ASPECTS.items()}
+    from tests._refgold import Store, norm, ref_path
+
+    def reference_classes():
+        ref = {}
+        for node in ast.parse(open(ref_path("tts/verifiers/openai_verifier.py")).read()).body:
+            if isinstance(node, ast.ClassDef) and node.name.startswith("Grading"):
+                tag = node.name[len("Grading_"):] or None
+                ref[tag] = list(s.target.id for s in node.body if isinstance(s, ast.AnnAssign))
+        return ref
+
+    ref = Store("verifier_adapters").value("grading_schemas", reference_classes)
+    assert ref == norm({k: list(v) for k, v in V.GRADING_ASPECTS.items()})
 
 
 def test_message_builders_equal_the_reference_methods():
     """openai_verifier.py:90-118, 166-238, 256-293: the three `prepare_*` methods of the reference's OpenAIVerifier
     (they do not touch `self`), compiled out of the reference source and fed the same images / strings as the
-    adapters here — the request payloads must be identical, JPEG bytes included."""
+    adapters here — the request payloads must be identical, JPEG bytes included (stored, tests/_refgold.py)."""
     import ast, base64
     from io import BytesIO
     from typing import Union
     from PIL import Image
-    path = "/root/reference/tts/verifiers/openai_verifier.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
-    ns = {"Union": Union, "Image": Image, "base64": base64, "BytesIO": BytesIO}
-    want = {"prepare_inputs", "prepare_refine_prompt_inputs", "prepare_reflexion_prompt_inputs"}
-    for node in ast.parse(open(path).read()).body:
-        if isinstance(node, ast.ClassDef) and node.name == "OpenAIVerifier":
-            for m in node.body:
-                if isinstance(m, ast.FunctionDef) and m.name in want:
-                    exec(compile(ast.Module([m], []), path, "exec"), ns)
-    assert want <= set(ns)
+    from tests._refgold import Store, norm, ref_path
     cands = [_cand(0, (200, 10, 30)), _cand(1, (5, 90, 250))]
     images = [c.pil() for c in cands]
     orig, cur = ["a red cube"] * 2, ["a red cube, studio light", "a red cube on a table"]
     refl, evals = ["make it redder", "center the cube"], ['{"overall_score": 7}', '{"overall_score": 3}']
     v = V.OpenAIShapedVerifier(FakeOpenAI(), "rubric")
     r = V.OpenAIShapedReflector(FakeOpenAI(), "REFLEX", "REFINE")
-    assert v.prepare_inputs(images, orig) == ns["prepare_inputs"](None, images, orig)
-    assert r.prepare_reflexion_prompt_inputs(images, orig, cur, refl, evals) == \
-        ns["prepare_reflexion_prompt_inputs"](None, images, orig, cur, refl, evals)
-    for kw in (dict(images=images, evaluations=evals, current_prompt=cur, reflections=refl),
-               dict(images=images, current_prompt=cur, reflections=refl),          # nvila branch: no evaluations
-               dict(images=images, evaluations=evals, current_prompt=cur),        # noise + prompt search: no reflections
-               dict()):
-        assert r.prepare_refine_prompt_inputs(orig, **kw) == ns["prepare_refine_prompt_inputs"](None, orig, **kw)
+    refine_kws = (dict(images=images, evaluations=evals, current_prompt=cur, reflections=refl),
+                  dict(images=images, current_prompt=cur, reflections=refl),          # nvila branch: no evaluations
+                  dict(images=images, evaluations=evals, current_prompt=cur),        # noise + prompt search: no reflections
+                  dict())
+
+    def reference_payloads():
+        path = ref_path("tts/verifiers/openai_verifier.py")
+        ns = {"Union": Union, "Image": Image, "base64": base64, "BytesIO": BytesIO}
+        want = {"prepare_inputs", "prepare_refine_prompt_inputs", "prepare_reflexion_prompt_inputs"}
+        for node in ast.parse(open(path).read()).body:
+            if isinstance(node, ast.ClassDef) and node.name == "OpenAIVerifier":
+                for m in node.body:
+                    if isinstance(m, ast.FunctionDef) and m.name in want:
+                        exec(compile(ast.Module([m], []), path, "exec"), ns)
+        assert want <= set(ns)
+        return {"inputs": ns["prepare_inputs"](None, images, orig),
+                "reflexion": ns["prepare_reflexion_prompt_inputs"](None, images, orig, cur, refl, evals),
+                "refine": [ns["prepare_refine_prompt_inputs"](None, orig, **kw) for kw in refine_kws]}
+
+    ref = Store("verifier_adapters").value("message_builders", reference_payloads)
+    assert norm(v.prepare_inputs(images, orig)) == ref["inputs"]
+    assert norm(r.prepare_reflexion_prompt_inputs(images, orig, cur, refl, evals)) == ref["reflexion"]
+    assert norm([r.prepare_refine_prompt_inputs(orig, **kw) for kw in refine_kws]) == ref["refine"]
 
 
 def test_reflection_generator_messages_equal_the_reference_function():
-    """tts_reflectionflow.py:27-41"""
+    """tts_reflectionflow.py:27-41 (the reference function's messages are stored, tests/_refgold.py)"""
     import ast
-    path = "/root/reference/tts/tts_reflectionflow.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
-    ns = {}
-    for node in ast.parse(open(path).read()).body:
-        if isinstance(node, ast.FunctionDef) and node.name == "generate_messages":
-            exec(compile(ast.Module([node], []), path, "exec"), ns)
-    for img, prompt in (("out/00001/midimg/2_round@17.png", 'a "quoted" prompt'), ("data:image/jpeg;base64,AAAA", "x")):
-        assert V.ReflectionGeneratorOurs.generate_messages(img, prompt) == ns["generate_messages"](img, prompt)
+    from tests._refgold import Store, norm, ref_path
+    cases = (("out/00001/midimg/2_round@17.png", 'a "quoted" prompt'), ("data:image/jpeg;base64,AAAA", "x"))
+
+    def reference_messages():
+        path = ref_path("tts/tts_reflectionflow.py")
+        ns = {}
+        for node in ast.parse(open(path).read()).body:
+            if isinstance(node, ast.FunctionDef) and node.name == "generate_messages":
+                exec(compile(ast.Module([node], []), path, "exec"), ns)
+        return [ns["generate_messages"](img, prompt) for img, prompt in cases]
+
+    ref = Store("verifier_adapters").value("generate_messages", reference_messages)
+    assert norm([V.ReflectionGeneratorOurs.generate_messages(img, prompt) for img, prompt in cases]) == ref
 
 
 def test_image_verifier_adapter_over_the_reference_reward_method():
     """reward_modeling/inference.py:71-76,155-180: the reference's `reward()` and `_norm()` methods, compiled out of
     the class and bound to a fake inferencer (model -> logits, no tokenizer / checkpoint), behind `ImageVerifierOurs`:
-    the adapter consumes exactly what the reference method returns, batch by batch, and ranks by `Overall` descending."""
+    the adapter consumes exactly what the reference method returns, batch by batch, and ranks by `Overall` descending.
+    What the reference method returned for each batch is stored (tests/_refgold.py) and replayed to the adapter."""
     import ast
-    path = "/root/reference/reward_modeling/inference.py"
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
-    ns = {}
-    for node in ast.parse(open(path).read()).body:
-        if isinstance(node, ast.ClassDef):
-            for m in node.body:
-                if isinstance(m, ast.FunctionDef) and m.name in ("reward", "_norm"):
-                    exec(compile(ast.Module([m], []), path, "exec"), ns)
-    assert {"reward", "_norm"} <= set(ns)
+    from tests._refgold import Store, norm, ref_path
     batches = []
 
-    class Inferencer:
+    class RecordingInferencer:  # the reference's methods bound to a fake model, run while recording
         inference_config = {"VQ_mean": 2.0, "VQ_std": 4.0}
-        reward = ns["reward"]
-        _norm = ns["_norm"]
+
+        def __init__(self):
+            ns = {}
+            for node in ast.parse(open(ref_path("reward_modeling/inference.py")).read()).body:
+                if isinstance(node, ast.ClassDef):
+                    for m in node.body:
+                        if isinstance(m, ast.FunctionDef) and m.name in ("reward", "_norm"):
+                            exec(compile(ast.Module([m], []), ref_path("reward_modeling/inference.py"), "exec"), ns)
+            assert {"reward", "_norm"} <= set(ns)
+            self._reward, self._norm_fn = ns["reward"], ns["_norm"]
+            self.calls = []
+
+        def _norm(self, *a, **k):
+            return self._norm_fn(self, *a, **k)
+
+        def reward(self, image_paths, prompts, **kw):
+            out = self._reward(self, image_paths, prompts, **kw)
+            self.calls.append({"n": len(image_paths), "kw": kw, "out": out})
+            return out
 
         def prepare_batch(self, image_paths, prompts, max_pixels):
-            batches.append(len(image_paths))
             return {"pix": [im.getpixel((0, 0))[0] for im in image_paths]}
 
         def model(self, return_dict, pix):
             return {"logits": torch.tensor([[float(p)] for p in pix])}
 
     cands = [_cand(i, (10 * i % 256, 0, 0)) for i in (5, 1, 9, 3, 7)]
+
+    def reference_calls():
+        inf = RecordingInferencer()
+        V.ImageVerifierOurs(inf, batch_size=2).score(cands, ["p"] * 5)
+        return inf.calls
+
+    calls = Store("verifier_adapters").value("image_verifier_reward", reference_calls)
+
+    class Inferencer:  # replays what the reference reward() returned, batch by batch
+        def reward(self, image_paths, prompts, **kw):
+            c = calls[len(batches)]
+            batches.append(len(image_paths))
+            assert c["n"] == len(image_paths) and c["kw"] == norm(kw)
+            return c["out"]
+
     v = V.ImageVerifierOurs(Inferencer(), batch_size=2)
     out = v.score(cands, ["p"] * 5)
     assert batches == [2, 2, 1]

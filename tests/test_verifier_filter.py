@@ -95,15 +95,13 @@ def test_main_walks_every_prompt_folder(tmp_path):
 def test_filter_equals_the_reference_main(tmp_path):
     """tts/verifier_filter.py::main (:28-176), unmodified, compiled out of its file and run over fakes (argument
     parser, NVILA loader, `Image.open(...).save(...)` recording paths) on the same run directory: the image copied
-    into every nfe<N> folder is the same."""
+    into every nfe<N> folder is the same (the reference's choices are stored, tests/_refgold.py)."""
     import ast
     import hashlib
     import types
 
     import numpy as np
-    ref_path = "/root/reference/tts/verifier_filter.py"
-    if not os.path.exists(ref_path):
-        pytest.skip("reference tree not present")
+    from tests._refgold import Store, ref_path
     run = tmp_path / "run"
     for i in range(2):
         f, _ = _make_run(str(tmp_path / f"tmp{i}"), rounds=(1, 2, 3, 10), per_round=5)   # 20 candidates: nfe32 = all
@@ -137,15 +135,19 @@ def test_filter_equals_the_reference_main(tmp_path):
             logits[0, 0 if label == "yes" else 1] = score
             return label, (logits,)
 
-    args = types.SimpleNamespace(pipeline_config_path=str(tmp_path / "cfg.json"), imgpath=str(run), start_index=0,
-                                 end_index=-1)
-    ns = dict(torch=torch, json=json, os=os, time=__import__("time"), Image=ImageMod, tqdm=lambda it, **kw: it,
-              parse_cli_args=lambda: args, load_model=lambda model_name, cache_dir: (Nvila, 0, 1))
-    fn = next(n for n in ast.parse(open(ref_path).read()).body if isinstance(n, ast.FunctionDef) and n.name == "main")
-    exec(compile(ast.Module([fn], []), ref_path, "exec"), ns)
-    ns["main"]()
-    ref_choice = {(os.path.basename(os.path.dirname(os.path.dirname(d))), os.path.basename(os.path.dirname(d))): s
-                  for d, s in saves}
+    def reference_choices():
+        path = ref_path("tts/verifier_filter.py")
+        args = types.SimpleNamespace(pipeline_config_path=str(tmp_path / "cfg.json"), imgpath=str(run), start_index=0,
+                                     end_index=-1)
+        ns = dict(torch=torch, json=json, os=os, time=__import__("time"), Image=ImageMod, tqdm=lambda it, **kw: it,
+                  parse_cli_args=lambda: args, load_model=lambda model_name, cache_dir: (Nvila, 0, 1))
+        fn = next(n for n in ast.parse(open(path).read()).body if isinstance(n, ast.FunctionDef) and n.name == "main")
+        exec(compile(ast.Module([fn], []), path, "exec"), ns)
+        ns["main"]()
+        return {os.path.basename(os.path.dirname(os.path.dirname(d))) + "/" + os.path.basename(os.path.dirname(d)):
+                os.path.relpath(s, run) for d, s in saves}
+
+    ref_choice = Store("verifier_filter").value("main", reference_choices)
 
     class Ours(StubVerifier):
         def score_one(self, cand, prompt):
@@ -155,4 +157,4 @@ def test_filter_equals_the_reference_main(tmp_path):
     for i in range(2):
         res = VF.filter_folder(str(run / f"{i:05}"), "a photo of a bench", Ours("nvila"), ctx=DistCtx())
         for n in VF.BUCKETS:
-            assert res["chosen"][n] + ".png" == ref_choice[(f"{i:05}", f"nfe{n}")], (i, n)
+            assert os.path.relpath(res["chosen"][n] + ".png", run) == ref_choice[f"{i:05}/nfe{n}"], (i, n)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline workload of BASELINE.json: FLUX-dev 1024x1024, 28 steps x 8 candidates x 4 reflection
+"""Headline workload: FLUX-dev 1024x1024, 28 steps x 8 candidates x 4 reflection
 rounds (entry B: 512x512 condition stream + LoRA), candidates sharded over the ranks, one all-gather of
 score records + one of candidate latents per round, VAE decode / resize / encode of every parent, stub
 verifier + reflector.  Prints one JSON line (rank 0).  torchrun-compatible."""

@@ -1,9 +1,11 @@
 // dev tool: MUFU.EX2 issue rate per SM sub-partition as a function of resident warps, and the
-// softmax-like instruction mix (FFMA2 + 2 MUFU + FADD2 + F2FP per 2 elements).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mufu_rate mufu_rate.cu && ./mufu_rate
+// softmax-like instruction mix (2 FFMA + 2 MUFU + 2 FADD + F2FP per 2 elements).
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mufu_rate mufu_rate.cu && ./mufu_rate
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float ex2(float x) { float y; asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 template <int MODE>
 __global__ void k(float* out, long long* cyc, int iters) {
@@ -21,9 +23,9 @@ __global__ void k(float* out, long long* cyc, int iters) {
     } else {
 #pragma unroll
       for (int i = 0; i < 16; i += 2) {
-        float2 x = __ffma2_rn(make_float2(v[i], v[i + 1]), make_float2(0.999f, 0.999f), make_float2(-0.01f, -0.01f));
+        float2 x = ffma2(make_float2(v[i], v[i + 1]), make_float2(0.999f, 0.999f), make_float2(-0.01f, -0.01f));
         float2 e; e.x = ex2(x.x); e.y = ex2(x.y);
-        acc = __fadd2_rn(acc, e);
+        acc = fadd2(acc, e);
         __nv_bfloat162 b = __floats2bfloat162_rn(e.x, e.y);
         pk ^= *reinterpret_cast<unsigned*>(&b);
         v[i] = x.x; v[i + 1] = x.y;
@@ -39,15 +41,15 @@ __global__ void k(float* out, long long* cyc, int iters) {
 }
 int main() {
   float* out; long long* cyc;
-  cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 148 * 8);
+  cudaMalloc(&out, 132 * 1024 * 4); cudaMalloc(&cyc, 132 * 8);
   const int iters = 2000;
   for (int mode = 0; mode < 2; ++mode)
     for (int threads : {32, 128, 256, 512, 1024}) {
       for (int rep = 0; rep < 2; ++rep) {
-        if (mode == 0) k<0><<<148, threads>>>(out, cyc, iters); else k<1><<<148, threads>>>(out, cyc, iters);
+        if (mode == 0) k<0><<<132, threads>>>(out, cyc, iters); else k<1><<<132, threads>>>(out, cyc, iters);
         cudaDeviceSynchronize();
       }
-      long long h[148]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
+      long long h[132]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
       double c = (double)h[0];
       int warps_per_smsp = threads <= 128 ? 1 : threads / 128;
       printf("mode %d threads %4d: %.0f cycles, %.2f cycles per MUFU warp-instr per SMSP (%d warp(s)/SMSP)\n", mode, threads, c,

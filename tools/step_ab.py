@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """dev tool: in-process A/B of launch-time switches on the denoise step (entry A 4608 tokens, entry B 5632 tokens
 exact LoRA), alternated in ONE process so that box / clock state is shared.  Switches are environment variables the
-library reads at graph-capture time:  python tools/step_ab.py RF_GEMM_EPI_GROUPS=2 RF_GEMM_EPI_GROUPS=1"""
+library reads at graph-capture time:  python tools/step_ab.py RF_SIDE_STREAM=1 RF_SIDE_STREAM=0"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
