@@ -60,9 +60,8 @@ int rf_op_linear(int epilogue, int M, int N, int K, const void* x, int ldx, cons
  * factors, RF_EPI_QKV); lora_B: [N, 64] (rank zero-padded).  M >= 128, N % 128 == 0, K % 64 == 0;
  * epilogues GELU / GATE_RES / QKV.  workspace: rf_op_linear_lora_workspace_bytes(M) bytes of device
  * memory (the bf16 down-projection lives there).  The down-projection runs as one GEMM launch with one
- * CTA per 128 x 64-column output tile (8-32 CTAs at M = 1024), full K per tile; the environment switch
- * RF_LORA_DOWN=side caps it at the four CTAs that rf_dit_forward / rf_dit_denoise fork onto a second
- * stream (same result). */
+ * CTA per 128 x 64-column output tile (8-24 CTAs at M = 1024), full K per tile; the product GEMM is one
+ * launch whose tiles each carry one extra 64-deep k-block for the low-rank term. */
 size_t rf_op_linear_lora_workspace_bytes(int M);
 int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx, const void* W,
                       const void* bias, void* y, int ldy, const void* lora_A, int t_cols,

@@ -127,10 +127,6 @@ struct rf_dit {
   cudaStream_t own_stream = nullptr;  // capture is illegal on the legacy default stream
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   int64_t graph_kernels = 0;  // kernel launches inside one captured step
-  // forked stream of the LoRA down-projections: they run on a few reserved SMs beside the other token streams'
-  // GEMM of the same layer (lora_down_side_launch) and join before the condition stream's launch
-  cudaStream_t side_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 };
 
 namespace {
@@ -511,48 +507,25 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     return rf::ln_modulate_launch(rowp(X, D, sr.row0), D, rowp(XN, D, sr.row0), D, sr.rows, D, scale,
                                   shift, sr.rows, 0, s);
   };
-  // RF_SIDE_STREAM=0 keeps the down-projections on the main stream (single-stream schedule; A/B of the fork)
-  const char* side_s = getenv("RF_SIDE_STREAM");  // read per enqueue (= per graph capture)
-  const bool side_env = !(side_s && atoi(side_s) == 0);
-  if (side_env && use_cond && !h->use_merged && h->any_lora && h->side_stream == nullptr) {
-    RF_CHECK_CUDA(cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
-  }
-  const bool side_lora = side_env && h->side_stream != nullptr;
   // A grouped GEMM whose LAST group is the condition stream carrying a LoRA (exact mode).  Fast path:
-  // T = bf16(x A^T) (one skinny GEMM), the other streams as one grouped launch, then the condition
-  // stream with the low-rank k-block fused (gemm2_lora_launch) — L = T B^T never reaches HBM.  Small /
+  // T = bf16(x A^T) (one skinny GEMM), then ONE grouped launch of all streams in which the condition
+  // stream's tiles carry the low-rank k-block (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Small /
   // odd shapes keep the unfused path: L materialised by two GEMMs and added in the epilogue (`addend`).
   // (t_pre != nullptr: T was already produced by an earlier launch, [M, ld_t] with this target's columns at t_pre)
   auto gemm_cond_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const bf16* loraA,
                             int t_cols, const bf16* loraB, int sec_cols, auto&& unfused_term,
                             const bf16* t_pre = nullptr, int ld_t = 0) -> int {
     rf::GemmGroupArgs& gc = gr[ngr - 1];
-    if (rf::gemm2_lora_eligible(epi, N, K, gc)) {
-      const bf16* T = t_pre;
-      if (T == nullptr && ngr > 1 && side_lora) {
-        // fork: the down-projection runs on kLoraSideCtas reserved SMs while the other streams' GEMM has the rest
-        RF_CHECK_CUDA(cudaEventRecord(h->ev_fork, s));
-        const int prev = rf::gemm_reserve_sms(rf::kLoraSideCtas);
-        const int mrc = rf::gemm_launch(epi, N, K, ngr - 1, gr, s);
-        rf::gemm_reserve_sms(prev);
-        if (mrc) return mrc;
-        RF_CHECK_CUDA(cudaStreamWaitEvent(h->side_stream, h->ev_fork, 0));
-        RF_TRY(rf::lora_down_side_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, h->side_stream));
-        RF_CHECK_CUDA(cudaEventRecord(h->ev_join, h->side_stream));
-        RF_CHECK_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-        return rf::gemm2_lora_launch(epi, N, K, gc, h->LT, t_cols, loraB, sec_cols, s);
-      }
-      if (T == nullptr) {
+    if (rf::gemm_lora_eligible(epi, N, K, gc)) {
+      if (t_pre == nullptr) {
         RF_TRY(rf::lora_down_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, s));
-        T = h->LT;
+        t_pre = h->LT;
         ld_t = t_cols;
       }
-      if (ngr > 1) RF_TRY(rf::gemm_launch(epi, N, K, ngr - 1, gr, s));
-      return rf::gemm2_lora_launch(epi, N, K, gc, T, ld_t, loraB, sec_cols, s);
+      gc.lora_T = t_pre; gc.ld_t = ld_t; gc.lora_B = loraB; gc.lora_sec_cols = sec_cols;
+    } else {
+      RF_TRY(unfused_term(gc));
     }
-    RF_TRY(unfused_term(gc));
     return rf::gemm_launch(epi, N, K, ngr, gr, s);
   };
   // all token streams of a norm in ONE launch: rows are [txt | img | cond] of the joint buffers
@@ -724,18 +697,15 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp in one launch (both GEMMs read the same XN rows)
     const bool t4 = use_cond && !h->use_merged && (b.l_q.set || b.l_k.set || b.l_v.set) && b.l_mlp.set &&
-                    rf::gemm2_lora_eligible(rf::EPI_QKV, D3, D, g[ng - 1]);
-    // (forked form: the launch of T happens inside gemm_cond_lora, with all 4 x 64 columns)
-    const bool t4_side = t4 && side_lora && ng > 1;
-    if (t4 && !t4_side)
+                    rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[ng - 1]);
+    if (t4)
       RF_TRY(rf::lora_down_launch(g[ng - 1].A, D, S_cond.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad, s));
     if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_QKV, D3, D, ng, g, b.qkvA, t4_side ? 4 * kLoraPad : 3 * kLoraPad, b.qkvB, D,
-                            [&](rf::GemmGroupArgs& gc) {
+      RF_TRY(gemm_cond_lora(rf::EPI_QKV, D3, D, ng, g, b.qkvA, 3 * kLoraPad, b.qkvB, D, [&](rf::GemmGroupArgs& gc) {
         RF_TRY(lora_term_qkv(h, b.qkvA, b.l_q, b.l_k, b.l_v, gc.A, D, S_cond.rows, h->LL, D3, s));
         gc.addend = h->LL; gc.ldadd = D3;
         return 0;
-      }, (t4 && !t4_side) ? h->LT : nullptr, 4 * kLoraPad));
+      }, t4 ? h->LT : nullptr, 4 * kLoraPad));
     } else {
       RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     }
@@ -952,9 +922,6 @@ void rf_dit_destroy(rf_dit* h) {
   if (h->own_stream) cudaStreamDestroy(h->own_stream);
   if (h->ev_in) cudaEventDestroy(h->ev_in);
   if (h->ev_out) cudaEventDestroy(h->ev_out);
-  if (h->side_stream) cudaStreamDestroy(h->side_stream);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
   for (void* p : h->allocs) cudaFree(p);
   delete h;
 }

@@ -30,8 +30,8 @@ static constexpr int kMaxGroups = 3;
 struct alignas(64) GemmGroupDev {
   CUtensorMap tmA;
   CUtensorMap tmB;
-  // fused peft LoRA (kLora kernels): T = bf16(x A^T) [M, 64 per section] and the B factor [N, 64];
-  // a tile in column section s = n0 / lora_sec_cols reads T columns [64 s, 64 s + 64)
+  // fused peft LoRA (groups with lora != 0, kLora kernels only): T = bf16(x A^T) [M, 64 per section] and
+  // the B factor [N, 64]; a tile in column section s = n0 / lora_sec_cols reads T columns [64 s, 64 s + 64)
   CUtensorMap tmT, tmLB;
   const bf16* bias;
   bf16* out;
@@ -48,6 +48,7 @@ struct alignas(64) GemmGroupDev {
   // out / res are [(H+2)(W+2), N]): an M tile is conv_by rows x conv_bx columns of OUTPUT pixels
   // (bx * by = 128); tap (ky, kx) of a k-block reads input pixels (s*y + ky + s-1, s*x + kx + s-1)
   int conv_w, conv_taps, conv_cin_blocks, conv_bx, conv_by, conv_stride;
+  int lora;  // this group's tiles carry the low-rank k-block (tmT, tmLB, lora_sec_cols)
 };
 
 struct alignas(64) GemmParamsDev {
@@ -130,7 +131,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
     for (int g = 0; g < p.ngroups; ++g) {
       tma_prefetch_desc(&p.g[g].tmA);
       tma_prefetch_desc(&p.g[g].tmB);
-      if constexpr (kLora) {
+      if (kLora && p.g[g].lora) {
         tma_prefetch_desc(&p.g[g].tmT);
         tma_prefetch_desc(&p.g[g].tmLB);
       }
@@ -156,12 +157,14 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
         const GemmGroupDev& G = p.g[tc.g];
         PixTile pt{0, 0};
         if (G.conv_w != 0) pt = pix_tile(G, tc.m0);
-        for (int kb = kLora ? -1 : 0; kb < p.num_kb; ++kb) {
+        // a LoRA group's tile carries one extra k-block after the main ones: T rows, B factor rows of the tile
+        const int kb_end = p.num_kb + ((kLora && G.lora) ? 1 : 0);
+        for (int kb = 0; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kStageBytesA;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          if (kLora && kb < 0) {  // the low-rank k-block first: T rows, B factor rows of the tile
+          if (kLora && kb == p.num_kb) {
             const int tcol = G.lora_sec_cols > 0 ? (tc.n0 / G.lora_sec_cols) * 64 : 0;
             tma_load_2d(sa, &G.tmT, &full_bar[stage], tcol, tc.m0);
             tma_load_2d(sb, &G.tmLB, &full_bar[stage], 0, tc.n0);
@@ -207,25 +210,6 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
     const TileCoord tc = decode_tile<BN>(p, t);
     const GemmGroupDev& G = p.g[tc.g];
 
-    // bf16(L) of the low-rank term, packed pairs in accumulator order (kLora)
-    uint32_t lpk[kLora ? BN / 4 : 1];
-    if constexpr (kLora) {
-      float accl[BN / 2];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) accl[i] = 0.f;
-      mbar_wait(&full_bar[stage], phase);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k) wgmma_tile<BN>(accl, a_desc(stage) + 2 * k, b_desc(stage) + 2 * k, k != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(accl);
-      release(stage);
-      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-#pragma unroll
-      for (int i = 0; i < BN / 4; ++i) lpk[i] = pack_bf16x2(accl[2 * i], accl[2 * i + 1]);
-    }
-
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -246,6 +230,34 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
     wgmma_wait<0>();
     fence_regs(acc);
     if (prev >= 0) release(prev);
+
+    // A LoRA group's tile: the low-rank k-block (T rows, B factor rows) follows in the ring.  It is multiplied
+    // one 128-column half at a time, right before that half's epilogue, so only a 64-register accumulator sits
+    // beside the main one; its slot is released after the last half.
+    const bool lora = kLora && G.lora;
+    const int lstage = stage;
+    if (lora) {
+      mbar_wait(&full_bar[stage], phase);
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    }
+    uint32_t lpk[kLora ? 32 : 1];  // bf16(L) of the current half, packed pairs in accumulator order
+    auto lora_half = [&](int hc) {
+      if constexpr (kLora) {
+        float accl[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) accl[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)  // B rows [128 hc, 128 hc + 128): + hc * 16 KB (encoded >> 4)
+          wgmma_ss_n128(accl, a_desc(lstage) + 2 * k, b_desc(lstage) + hc * 1024 + 2 * k, k != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(accl);
+        if (hc == BN / 128 - 1) release(lstage);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) lpk[i] = pack_bf16x2(accl[2 * i], accl[2 * i + 1]);
+      }
+    };
 
     // ===================== epilogue: registers -> fused math -> HBM =====================
     // this thread: rows r_loc + {0, 8} of the tile, columns 8 j + cq + {0, 1}
@@ -284,10 +296,12 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
         bf16_round2(v0, v1);
       }
       if constexpr (kLora) {
-        const float2 l = unpack_bf16x2(lpk[2 * j + h2]);
-        v0 += l.x;
-        v1 += l.y;
-        bf16_round2(v0, v1);
+        if (lora) {
+          const float2 l = unpack_bf16x2(lpk[2 * (j % 16) + h2]);  // j inside the half lora_half() left in lpk
+          v0 += l.x;
+          v1 += l.y;
+          bf16_round2(v0, v1);
+        }
       }
     };
     auto store = [&](int j, int h2, float v0, float v1) {
@@ -304,6 +318,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
       for (int hc = 0; hc < BN / 128; ++hc) {
         const int col_h = tc.n0 + hc * 128;
         const int section = col_h / inner;  // 0 q, 1 k, 2 v
+        if (lora) lora_half(hc);
         float v[2][32];
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
@@ -348,6 +363,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = tc.n0 + 8 * j + cq;
+        if (lora && j % 16 == 0) lora_half(j / 16);
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           float v0, v1;
@@ -471,38 +487,29 @@ int gemm_init() {
   rc |= set_attr<128, EPI_GATE_RES, false>(); rc |= set_attr<128, EPI_QKV, false>();
   rc |= set_attr<64, EPI_BIAS, false>(); rc |= set_attr<64, EPI_GELU, false>();
   rc |= set_attr<64, EPI_GATE_RES, false>();
+  rc |= set_attr<256, EPI_GELU, true>(); rc |= set_attr<256, EPI_GATE_RES, true>();
+  rc |= set_attr<256, EPI_QKV, true>();
   rc |= set_attr<128, EPI_GELU, true>(); rc |= set_attr<128, EPI_GATE_RES, true>();
   rc |= set_attr<128, EPI_QKV, true>();
   return rc ? -2 : 0;
 }
 
-static thread_local int g_reserve_sms = 0;
-int gemm_reserve_sms(int sms) {
-  const int prev = g_reserve_sms;
-  g_reserve_sms = sms < 0 ? 0 : sms;
-  return prev;
-}
-// persistent grid: one CTA per SM, minus the reserved ones when the tiles still take the same number of
-// waves; max_ctas > 0 caps it (the LoRA down-projection that runs beside another GEMM)
-static int grid_ctas(int tiles, int max_ctas) {
-  int ctas = num_sms();
-  const int fewer = ctas - g_reserve_sms;
-  if (g_reserve_sms > 0 && fewer > 0 && (tiles + fewer - 1) / fewer == (tiles + ctas - 1) / ctas) ctas = fewer;
-  if (max_ctas > 0 && ctas > max_ctas) ctas = max_ctas;
-  if (ctas > tiles) ctas = tiles;
-  return ctas;
+// persistent grid: one CTA per SM
+static int grid_ctas(int tiles) {
+  const int ctas = num_sms();
+  return ctas > tiles ? tiles : ctas;
 }
 
 template <int BN, int EPI, bool LORA>
-static int launch_cfg(GemmParamsDev& p, int max_ctas, cudaStream_t stream) {
+static int launch_cfg(GemmParamsDev& p, const char* name, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
   if (int rc = set_attr<BN, EPI, LORA>()) return rc;
-  const int grid = grid_ctas(p.total_tiles, max_ctas);
+  const int grid = grid_ctas(p.total_tiles);
   double rows = 0;
   for (int g = 0; g < p.ngroups; ++g) rows += p.g[g].M;
   static const char* kNames[4] = {"gemm_bias", "gemm_gelu", "gemm_gate_res", "gemm_qkv_rms_rope"};
   const bool conv = p.g[0].conv_w != 0;
-  const char* name = conv ? (EPI == EPI_GATE_RES ? "conv_res" : "conv_bias") : kNames[EPI];
+  if (name == nullptr) name = conv ? (EPI == EPI_GATE_RES ? "conv_res" : "conv_bias") : kNames[EPI];
   // algorithmic FLOPs: 2 M N K; algorithmic bytes: A (each pixel once for a convolution) + W + out once
   ProfScope prof(name, 2.0 * rows * p.N * p.K,
                  2.0 * (rows * p.K / (conv ? p.g[0].conv_taps : 1) +
@@ -514,16 +521,25 @@ static int launch_cfg(GemmParamsDev& p, int max_ctas, cudaStream_t stream) {
   return 0;
 }
 
-template <int BN>
-static int launch_bn(int epi, GemmParamsDev& p, int max_ctas, cudaStream_t stream) {
-  switch (epi) {
-    case EPI_BIAS: return launch_cfg<BN, EPI_BIAS, false>(p, max_ctas, stream);
-    case EPI_GELU: return launch_cfg<BN, EPI_GELU, false>(p, max_ctas, stream);
-    case EPI_GATE_RES: return launch_cfg<BN, EPI_GATE_RES, false>(p, max_ctas, stream);
-    case EPI_QKV:
-      if constexpr (BN >= 128) return launch_cfg<BN, EPI_QKV, false>(p, max_ctas, stream);
-      break;
-    default: break;
+template <int BN, bool LORA>
+static int launch_bn(int epi, GemmParamsDev& p, const char* name, cudaStream_t stream) {
+  if constexpr (LORA) {  // the low-rank term is fused after a bias rounding: not offered for EPI_BIAS
+    switch (epi) {
+      case EPI_GELU: return launch_cfg<BN, EPI_GELU, true>(p, name, stream);
+      case EPI_GATE_RES: return launch_cfg<BN, EPI_GATE_RES, true>(p, name, stream);
+      case EPI_QKV: return launch_cfg<BN, EPI_QKV, true>(p, name, stream);
+      default: break;
+    }
+  } else {
+    switch (epi) {
+      case EPI_BIAS: return launch_cfg<BN, EPI_BIAS, false>(p, name, stream);
+      case EPI_GELU: return launch_cfg<BN, EPI_GELU, false>(p, name, stream);
+      case EPI_GATE_RES: return launch_cfg<BN, EPI_GATE_RES, false>(p, name, stream);
+      case EPI_QKV:
+        if constexpr (BN >= 128) return launch_cfg<BN, EPI_QKV, false>(p, name, stream);
+        break;
+      default: break;
+    }
   }
   set_error("gemm_launch: epilogue not available for this tile width");
   return -1;
@@ -536,7 +552,16 @@ static void set_raster(GemmParamsDev& p) { p.band = p.n_tiles <= 12 ? p.n_tiles 
 static bool g_narrow_tiles = false;
 void dbg_force_gemm_v1(bool on) { g_narrow_tiles = on; }
 
-static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups, int max_ctas,
+bool gemm_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a) {
+  if (epi != EPI_GELU && epi != EPI_GATE_RES && epi != EPI_QKV) return false;
+  if (N % 128 != 0 || K % BK != 0 || a.M < 128 || a.addend != nullptr) return false;
+  if (epi == EPI_QKV && N % 384 != 0) return false;
+  if ((a.ldo * 2) % 16 != 0 || (reinterpret_cast<uintptr_t>(a.out) & 15)) return false;
+  if (epi == EPI_GATE_RES && ((a.ldr * 2) % 16 != 0 || (reinterpret_cast<uintptr_t>(a.res) & 15))) return false;
+  return true;
+}
+
+static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups, const char* name,
                             cudaStream_t stream) {
   if (ngroups < 1 || ngroups > kMaxGroups) {
     set_error("gemm_launch: ngroups must be 1..3");
@@ -554,6 +579,21 @@ static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupA
   if (epi == EPI_QKV && (bn < 128 || N % 384 != 0)) {
     set_error("gemm_launch: EPI_QKV needs N = 3 * heads * 128");
     return -1;
+  }
+  bool lora = false;
+  for (int g = 0; g < ngroups; ++g) {
+    const GemmGroupArgs& a = groups[g];
+    if (a.lora_T == nullptr) continue;
+    if (a.lora_B == nullptr || !gemm_lora_eligible(epi, N, K, a) ||
+        (a.lora_sec_cols > 0 && (a.lora_sec_cols % 128 != 0 || N % a.lora_sec_cols != 0))) {
+      set_error("gemm_launch: LoRA group needs M >= 128, N % 128 == 0 (QKV: N % 384 == 0), 16-byte aligned "
+                "out / res pitches, no addend, sections of a multiple of 128 columns, and the GELU / GATE_RES / "
+                "QKV epilogue");
+      return -1;
+    }
+    // a tile reads the T columns of one section: 256-wide tiles only when they cannot straddle one
+    if (a.lora_sec_cols % 256 != 0) bn = 128;
+    lora = true;
   }
   // 256-wide tiles halve the W traffic per FLOP; narrower ones when 256-wide tiles would leave SMs idle
   if (bn == 256) {
@@ -585,6 +625,15 @@ static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupA
     if (rc) return rc;
     rc = make_tmap_2d(&d.tmB, a.W, N, K, K, bn);
     if (rc) return rc;
+    if (a.lora_T != nullptr) {
+      const int t_cols = a.lora_sec_cols > 0 ? (N / a.lora_sec_cols) * 64 : 64;
+      rc = make_tmap_2d(&d.tmT, a.lora_T, a.M, t_cols, a.ld_t, BM);
+      if (rc) return rc;
+      rc = make_tmap_2d(&d.tmLB, a.lora_B, N, 64, 64, bn);
+      if (rc) return rc;
+      d.lora = 1;
+      d.lora_sec_cols = a.lora_sec_cols;
+    }
     d.bias = a.bias; d.out = a.out; d.addend = a.addend; d.res = a.res; d.gate = a.gate;
     d.rope_cos = a.rope_cos; d.rope_sin = a.rope_sin; d.norm_q = a.norm_q; d.norm_k = a.norm_k;
     d.M = a.M; d.ldo = a.ldo; d.ldadd = a.ldadd; d.ldr = a.ldr;
@@ -601,88 +650,27 @@ static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupA
     }
   }
   p.total_tiles = tiles;
+  if (lora) {
+    return bn == 256 ? launch_bn<256, true>(epi, p, name, stream) : launch_bn<128, true>(epi, p, name, stream);
+  }
   switch (bn) {
-    case 256: return launch_bn<256>(epi, p, max_ctas, stream);
-    case 128: return launch_bn<128>(epi, p, max_ctas, stream);
-    default: return launch_bn<64>(epi, p, max_ctas, stream);
+    case 256: return launch_bn<256, false>(epi, p, name, stream);
+    case 128: return launch_bn<128, false>(epi, p, name, stream);
+    default: return launch_bn<64, false>(epi, p, name, stream);
   }
 }
 
 int gemm_launch(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups, cudaStream_t stream) {
-  return gemm_launch_impl(epi, N, K, ngroups, groups, 0, stream);
+  return gemm_launch_impl(epi, N, K, ngroups, groups, nullptr, stream);
 }
 
 // ---- LoRA down-projection: T[M, NT] = bf16(X[M, K] @ A[NT, K]^T), an EPI_BIAS GEMM without bias
-static GemmGroupArgs lora_down_args(const bf16* X, int ldx, int M, const bf16* A, bf16* T, int ldT) {
+int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
+                     cudaStream_t stream) {
   GemmGroupArgs g;
   memset(&g, 0, sizeof(g));
   g.A = X; g.lda = ldx; g.M = M; g.W = A; g.out = T; g.ldo = ldT;
-  return g;
-}
-int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
-                     cudaStream_t stream) {
-  const GemmGroupArgs g = lora_down_args(X, ldx, M, A, T, ldT);
-  return gemm_launch_impl(EPI_BIAS, NT, K, 1, &g, 0, stream);
-}
-int lora_down_side_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
-                          cudaStream_t stream) {
-  const GemmGroupArgs g = lora_down_args(X, ldx, M, A, T, ldT);
-  return gemm_launch_impl(EPI_BIAS, NT, K, 1, &g, kLoraSideCtas, stream);
-}
-
-// ---- one token stream with peft LoRA fused: out = epi(bf16(bf16(A W^T + b) + bf16(T B^T)))
-bool gemm2_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a) {
-  if (epi != EPI_GELU && epi != EPI_GATE_RES && epi != EPI_QKV) return false;
-  if (N % 128 != 0 || K % BK != 0 || a.M < 128 || a.addend != nullptr) return false;
-  if (epi == EPI_QKV && N % 384 != 0) return false;
-  if ((a.ldo * 2) % 16 != 0 || (reinterpret_cast<uintptr_t>(a.out) & 15)) return false;
-  if (epi == EPI_GATE_RES && ((a.ldr * 2) % 16 != 0 || (reinterpret_cast<uintptr_t>(a.res) & 15))) return false;
-  return true;
-}
-int gemm2_lora_launch(int epi, int N, int K, const GemmGroupArgs& a, const bf16* T, int ldT,
-                      const bf16* loraB, int sec_cols, cudaStream_t stream) {
-  constexpr int bn = 128;  // two fp32 accumulators (base + low-rank) per thread
-  GemmParamsDev p;
-  memset(&p, 0, sizeof(p));
-  p.ngroups = 1;
-  p.N = N;
-  p.K = K;
-  p.n_tiles = N / bn;
-  p.num_kb = K / BK;
-  set_raster(p);
-  GemmGroupDev& d = p.g[0];
-  int rc = make_tmap_2d(&d.tmA, a.A, a.M, K, a.lda, BM);
-  if (rc) return rc;
-  rc = make_tmap_2d(&d.tmB, a.W, N, K, K, bn);
-  if (rc) return rc;
-  const int t_cols = sec_cols > 0 ? (N / sec_cols) * 64 : 64;
-  rc = make_tmap_2d(&d.tmT, T, a.M, t_cols, ldT, BM);
-  if (rc) return rc;
-  rc = make_tmap_2d(&d.tmLB, loraB, N, 64, 64, bn);
-  if (rc) return rc;
-  if (epi == EPI_GATE_RES && (a.res == nullptr || a.gate == nullptr)) {
-    set_error("gemm2_lora_launch: EPI_GATE_RES needs res and gate");
-    return -1;
-  }
-  if (epi == EPI_QKV && (!a.rope_cos || !a.rope_sin || !a.norm_q || !a.norm_k)) {
-    set_error("gemm2_lora_launch: EPI_QKV needs rope tables and norm weights");
-    return -1;
-  }
-  d.bias = a.bias; d.out = a.out; d.addend = nullptr; d.res = a.res; d.gate = a.gate;
-  d.rope_cos = a.rope_cos; d.rope_sin = a.rope_sin; d.norm_q = a.norm_q; d.norm_k = a.norm_k;
-  d.M = a.M; d.ldo = a.ldo; d.ldadd = 0; d.ldr = a.ldr;
-  d.lora_sec_cols = sec_cols;
-  d.m_tiles = (a.M + BM - 1) / BM;
-  d.tile_begin = 0;
-  p.total_tiles = d.m_tiles * p.n_tiles;
-  switch (epi) {
-    case EPI_GELU: return launch_cfg<bn, EPI_GELU, true>(p, 0, stream);
-    case EPI_GATE_RES: return launch_cfg<bn, EPI_GATE_RES, true>(p, 0, stream);
-    case EPI_QKV: return launch_cfg<bn, EPI_QKV, true>(p, 0, stream);
-    default: break;
-  }
-  set_error("gemm2_lora_launch: unsupported epilogue");
-  return -1;
+  return gemm_launch_impl(EPI_BIAS, NT, K, 1, &g, "lora_down", stream);
 }
 
 // 3x3 (taps = 9) or 1x1 (taps = 1) convolution, stride 1 (zero padding 1) or stride 2 (diffusers
@@ -733,7 +721,7 @@ int conv_launch(const bf16* in, const bf16* weight, const bf16* bias, bf16* out,
   d.conv_stride = stride;
   p.total_tiles = d.m_tiles * p.n_tiles;
   const int epi = res ? EPI_GATE_RES : EPI_BIAS;
-  return bn == 256 ? launch_bn<256>(epi, p, 0, stream) : launch_bn<128>(epi, p, 0, stream);
+  return bn == 256 ? launch_bn<256, false>(epi, p, nullptr, stream) : launch_bn<128, false>(epi, p, nullptr, stream);
 }
 
 }  // namespace rf

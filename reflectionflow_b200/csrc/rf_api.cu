@@ -162,7 +162,7 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
   g.rope_cos = rope_cos; g.rope_sin = rope_sin;
   g.norm_q = static_cast<const bf16*>(norm_q);
   g.norm_k = static_cast<const bf16*>(norm_k);
-  if (!rf::gemm2_lora_eligible(epilogue, N, K, g)) {
+  if (!rf::gemm_lora_eligible(epilogue, N, K, g)) {
     rf::set_error("rf_op_linear_lora: needs M >= 128, N % 128 == 0 (QKV: N % 384 == 0), K % 64 == 0, "
                   "16-byte aligned pitches, and the GELU / GATE_RES / QKV epilogue");
     return -1;
@@ -170,14 +170,12 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // workspace = T (bf16 [rows, t_cols])
   bf16* T = static_cast<bf16*>(workspace);
-  // RF_LORA_DOWN=side: the confined few-CTA form the DiT forks beside its main GEMM (here on the caller's stream)
-  const char* form = getenv("RF_LORA_DOWN");
-  int rc = (form && strcmp(form, "side") == 0)
-               ? rf::lora_down_side_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, s)
-               : rf::lora_down_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, s);
+  int rc = rf::lora_down_launch(g.A, ldx, M, K, static_cast<const bf16*>(lora_A), t_cols, T, t_cols, s);
   if (rc) return rc;
-  return rf::gemm2_lora_launch(epilogue, N, K, g, T, t_cols, static_cast<const bf16*>(lora_B),
-                               t_cols == 192 ? N / 3 : 0, s);
+  g.lora_T = T; g.ld_t = t_cols;
+  g.lora_B = static_cast<const bf16*>(lora_B);
+  g.lora_sec_cols = t_cols == 192 ? N / 3 : 0;
+  return rf::gemm_launch(epilogue, N, K, 1, &g, s);
 }
 
 int rf_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out,

@@ -90,30 +90,24 @@ struct GemmGroupArgs {
   const float* rope_sin;
   const bf16* norm_q;              // EPI_QKV: [128]
   const bf16* norm_k;
+  // peft's unfused LoRA arithmetic fused into this group's tiles (lora_T != nullptr):
+  //   out = epi( bf16( bf16(A W^T + b) + bf16(T lora_B^T) ) ),  T = bf16(A loraA^T) computed beforehand.
+  // T: [M, ld_t]; with lora_sec_cols > 0 output section s = n / lora_sec_cols reads T columns
+  // [64 s, 64 s + 64) (stacked q|k|v); lora_B: [N, 64] (rank zero-padded to 64).  See gemm_lora_eligible.
+  const bf16* lora_T; int ld_t;
+  const bf16* lora_B;
+  int lora_sec_cols;
 };
 int gemm_launch(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups,
                 cudaStream_t stream);
 
-// One token stream with peft's unfused LoRA arithmetic fused into the GEMM (gemm_sm90.cu, kLora):
-//   out = epi( bf16( bf16(A W^T + b) + bf16(T loraB^T) ) ),  T = bf16(A loraA^T) computed beforehand.
-// T: [M, ldT]; with sec_cols > 0 output section s = n / sec_cols reads T columns [64 s, 64 s + 64)
-// (stacked q|k|v); loraB: [N, 64] (rank zero-padded to 64).
-bool gemm2_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a);
-int gemm2_lora_launch(int epi, int N, int K, const GemmGroupArgs& a, const bf16* T, int ldT,
-                      const bf16* loraB, int sec_cols, cudaStream_t stream);
+// Whether group `a` (without its lora_* fields) can carry the fused LoRA term in gemm_launch.
+bool gemm_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a);
 
 // LoRA down-projection of one token stream: T[M, NT] = bf16(X[M, K] @ A[NT, K]^T), NT a multiple of 64,
 // on the GEMM kernel above (fp32 accumulation over the whole K, one rounding).
 int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
                      cudaStream_t stream);
-// The same product on kLoraSideCtas SMs only, for a forked stream that runs beside a GEMM launched with
-// gemm_reserve_sms(kLoraSideCtas).
-static constexpr int kLoraSideCtas = 4;
-int lora_down_side_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
-                          cudaStream_t stream);
-// The next GEMM launches of this thread leave `sms` SMs free when that does not add a wave of tiles
-// (0 = use every SM).  Returns the previous value.
-int gemm_reserve_sms(int sms);
 
 // ---------------------------------------------------------------------------- attention
 // Non-causal softmax(Q K^T / sqrt(128)) V over one joint token sequence.
