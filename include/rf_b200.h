@@ -74,7 +74,7 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
  * F.scaled_dot_product_attention at train_flux/flux/block.py:123-125 (plus the cat/transpose
  * around it).  cond_mode: 0 = plain; 1 = additive bias `cond_bias` between tokens [0,n_main)
  * and [n_main,n_tok) (attn.c_factor, block.py:115-122); 2 = those cross blocks masked out
- * (union_cond_attn = False, block.py:106-114). */
+ * (union_cond_attn = False, block.py:106-114).  With cond_mode != 0, 0 < n_main < n_tok (any split). */
 int rf_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out,
                     int n_tok, int heads, int batch, int n_main, int cond_mode, float cond_bias,
                     void* stream);
@@ -191,14 +191,15 @@ int rf_vae_missing_weights(rf_vae* h);
 /* packed latents [(H/16)(W/16), 64] bf16 (one image) -> image.  Applies
  * `latents / scaling_factor + shift_factor` (bf16 ops), the decoder, and
  * VaeImageProcessor.postprocess: out_u8_hwc [H, W, 3] uint8 and/or out_bf16_chw [3, H, W] bf16
- * (either may be NULL).  width % 1024 == 0, height % 16 == 0. */
+ * (either may be NULL).  height, width: multiples of 16 in [16, 16384]; the workspace (grown on demand, the
+ * mid-block's (H/8 * W/8)^2 bf16 scores dominate it) must fit on the device. */
 int rf_vae_decode(rf_vae* h, const void* packed_latents, int height, int width, float scaling_factor,
                   float shift_factor, uint8_t* out_u8_hwc, void* out_bf16_chw, void* stream);
 /* encode_images() of train_flux/flux/pipeline_tools.py:7-30 (Condition.encode, condition.py:96-132):
  * image [H, W, 3] uint8 (or bf16 [3, H, W] already in [-1, 1]; exactly one non-NULL) ->
  * VaeImageProcessor.preprocess -> encoder -> posterior sample mean + std * eps with CALLER-PROVIDED
  * eps (bf16 [16, H/8, W/8]; NULL = posterior mode; the reference draws eps from the global RNG)
- * -> (z - shift) * scaling -> packed tokens [(H/16)(W/16), 64] bf16. */
+ * -> (z - shift) * scaling -> packed tokens [(H/16)(W/16), 64] bf16.  Sizes as for rf_vae_decode. */
 int rf_vae_encode(rf_vae* h, const uint8_t* image_u8_hwc, const void* image_bf16_chw, int height,
                   int width, const void* eps_bf16_chw, float scaling_factor, float shift_factor,
                   void* packed_out, void* stream);

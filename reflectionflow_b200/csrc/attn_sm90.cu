@@ -12,7 +12,8 @@
 //   warpgroups 1, 2  query rows [0, 64) / [64, 128): S = Q K^T by wgmma (both operands from shared
 //                    memory), online softmax in registers (log2 domain), P packed to bf16 in registers
 //                    and O += P V by wgmma with P as the register A operand (V read MN-major)
-// A masked (q tile, kv tile) pair of cond_mode 2 is skipped: its P would be 0.
+// A masked (q tile, kv tile) pair of cond_mode 2 is skipped: its P would be 0.  When n_main % 128 != 0 the query
+// tile and the kv tile that hold the split take the cond_mode 2 mask / cond_mode 1 bias per element instead.
 #include <cuda.h>
 
 #include "rf_internal.h"
@@ -34,6 +35,7 @@ struct alignas(64) AttnParamsDev {
   int n_main, cond_mode;
   float scale_log2;  // log2(e) / sqrt(128)
   float bias_log2;   // log2(e) * cond_bias
+  float bias_raw;    // cond_bias * sqrt(128): the same bias added to a raw score (split tiles)
 };
 
 __device__ __forceinline__ float ex2_approx(float x) {
@@ -115,6 +117,9 @@ attn_kernel(const __grid_constant__ AttnParamsDev p) {
   const int wq = (threadIdx.x >> 5) & 3;
   const int cq = 2 * (lane & 3);
   const bool q_is_cond = (p.cond_mode != 0) && (q0 >= p.n_main);
+  // the query tile holding the split row n_main (n_main % 128 != 0): rows on both sides of it
+  const bool q_straddle = (p.cond_mode != 0) && q0 < p.n_main && p.n_main < q0 + kTile;
+  const int row0 = q0 + cw * 64 + wq * 16 + (lane >> 2);  // this thread's query rows: row0, row0 + 8
   const uint32_t aQ = smem_u32(sQ) + cw * 64 * 128, aK = smem_u32(sK), aV = smem_u32(sV);
 
   float o[64];
@@ -132,13 +137,15 @@ attn_kernel(const __grid_constant__ AttnParamsDev p) {
     const int st = j & 1;
     const uint32_t ph = (j >> 1) & 1;
     const bool cross = (p.cond_mode != 0) && ((j * kTile >= p.n_main) != q_is_cond);
+    // a pair with the split inside its query or its key range takes the mask / bias per element
+    const bool split = q_straddle || ((p.cond_mode != 0) && j * kTile < p.n_main && p.n_main < (j + 1) * kTile);
     mbar_wait(&k_full[st], ph);
-    if (p.cond_mode == 2 && cross) {  // fully masked tile: P = 0, statistics untouched
+    if (p.cond_mode == 2 && cross && !split) {  // fully masked tile: P = 0, statistics untouched
       mbar_wait(&v_full[st], ph);
       release(st);
       continue;
     }
-    const float bias = (p.cond_mode == 1 && cross) ? p.bias_log2 : 0.f;
+    const float bias = (p.cond_mode == 1 && cross && !split) ? p.bias_log2 : 0.f;
     float s[64];
     wgmma_fence();
 #pragma unroll
@@ -163,6 +170,23 @@ attn_kernel(const __grid_constant__ AttnParamsDev p) {
             s[4 * jj + 2 + e] = -INFINITY;
           }
     }
+    if (split) {
+      // per element: -inf where cond_mode 2 masks the pair, + cond_bias (in units of the raw score) where
+      // cond_mode 1 biases it; the statistics below then run with no tile bias
+      const int kc = p.n_main - j * kTile - cq;  // key column 8 jj + e is a condition key iff 8 jj + e >= kc
+#pragma unroll
+      for (int h2 = 0; h2 < 2; ++h2) {
+        const bool rc = row0 + 8 * h2 >= p.n_main;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if ((8 * jj + e >= kc) != rc) {
+              float& v = s[4 * jj + 2 * h2 + e];
+              v = p.cond_mode == 2 ? -INFINITY : v + p.bias_raw;
+            }
+      }
+    }
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int jj = 0; jj < 16; ++jj)
@@ -175,7 +199,10 @@ attn_kernel(const __grid_constant__ AttnParamsDev p) {
       mx[h2] = fmaxf(mx[h2], __shfl_xor_sync(0xffffffffu, mx[h2], 1));
       mx[h2] = fmaxf(mx[h2], __shfl_xor_sync(0xffffffffu, mx[h2], 2));
       const float m_new = fmaxf(m_run[h2], fmaf(mx[h2], p.scale_log2, bias));
-      const float alpha = ex2_approx(m_run[h2] - m_new);  // 0 on the first tile
+      // split pairs only: a row whose keys so far are all masked keeps max -inf but exponentiates against 0
+      // (-inf - -inf would be NaN); its P, O and row sum stay 0
+      const float m_use = (split && m_new == -INFINITY) ? 0.f : m_new;
+      const float alpha = ex2_approx(m_run[h2] - m_use);  // 0 on the first tile
       m_run[h2] = m_new;
       l_run[h2] *= alpha;
 #pragma unroll
@@ -183,7 +210,7 @@ attn_kernel(const __grid_constant__ AttnParamsDev p) {
         o[4 * jj + 2 * h2] *= alpha;
         o[4 * jj + 2 * h2 + 1] *= alpha;
       }
-      neg_m[h2] = bias - m_new;
+      neg_m[h2] = bias - m_use;
     }
     // P = exp2(s * scale + bias - m), packed into the A fragments of the 8 k-steps of P V
     uint32_t pa[8][4];
@@ -242,8 +269,8 @@ int attention_launch(const AttnArgs& a, cudaStream_t stream) {
     set_error("attention_launch: empty problem");
     return -1;
   }
-  if (a.cond_mode != 0 && (a.n_main % kTile != 0 || a.n_main <= 0 || a.n_main >= a.n_tok)) {
-    set_error("attention_launch: cond split must be a positive multiple of 128 below n_tok");
+  if (a.cond_mode != 0 && (a.n_main <= 0 || a.n_main >= a.n_tok)) {
+    set_error("attention_launch: cond split must lie inside (0, n_tok)");
     return -1;
   }
   if (a.batch > 1 && a.n_tok % kTile != 0) {
@@ -276,6 +303,7 @@ int attention_launch(const AttnArgs& a, cudaStream_t stream) {
   const float kLog2e = 1.4426950408889634f;
   p.scale_log2 = kLog2e * 0.08838834764831845f;  // 1/sqrt(128)
   p.bias_log2 = kLog2e * a.cond_bias;
+  p.bias_raw = a.cond_bias * 11.313708498984761f;  // sqrt(128)
   if (int rc = attention_init()) return rc;
   const int grid = p.q_tiles * a.heads * a.batch;
   // algorithmic FLOPs: QK^T and PV only (4 * n^2 * 128 per head); bytes: q,k,v read + o written

@@ -1031,10 +1031,6 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     }
     if (flags & 4) mode = 2;  // union_cond_attn == False wins only if no c_factor...
     if ((flags & 4) && condition_scale != 1.0f) mode = 1;  // c_factor mask overrides (block.py:115)
-    if (mode != 0 && n_main % 128 != 0) {
-      rf::set_error("rf_dit_prepare: cond attention modes need (n_txt + n_img) % 128 == 0");
-      return -1;
-    }
   }
   const bool same = h->prepared && h->batch == batch && h->n_txt == n_txt && h->n_img == n_img &&
                     h->n_cond == n_cond;

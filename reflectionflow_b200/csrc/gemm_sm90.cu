@@ -46,8 +46,10 @@ struct alignas(64) GemmGroupDev {
   int m_tiles, tile_begin, lora_sec_cols;
   // implicit-GEMM convolution over zero-ringed NHWC images (conv_w > 0; tmA is a 3-D map {C, W+2, H+2},
   // out / res are [(H+2)(W+2), N]): an M tile is conv_by rows x conv_bx columns of OUTPUT pixels
-  // (bx * by = 128); tap (ky, kx) of a k-block reads input pixels (s*y + ky + s-1, s*x + kx + s-1)
-  int conv_w, conv_taps, conv_cin_blocks, conv_bx, conv_by, conv_stride;
+  // (bx * by = 128), conv_xt tiles per row of tiles; tap (ky, kx) of a k-block reads input pixels
+  // (s*y + ky + s-1, s*x + kx + s-1).  Tiles of the last column / row may reach past W / H: TMA zero-fills
+  // the reads outside the ringed input and the epilogue skips those pixels.
+  int conv_w, conv_h, conv_xt, conv_taps, conv_cin_blocks, conv_bx, conv_by, conv_stride;
   int lora;  // this group's tiles carry the low-rank k-block (tmT, tmLB, lora_sec_cols)
 };
 
@@ -97,10 +99,9 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmParamsDev& p, int t) 
 
 struct PixTile { int x0, y0; };
 __device__ __forceinline__ PixTile pix_tile(const GemmGroupDev& G, int m0) {
-  const int mt = m0 >> 7;                // 128-pixel tile index
-  const int xt = G.conv_w / G.conv_bx;   // tiles per image row
-  const int ty = mt / xt;
-  return PixTile{(mt - ty * xt) * G.conv_bx, ty * G.conv_by};
+  const int mt = m0 >> 7;  // 128-pixel tile index
+  const int ty = mt / G.conv_xt;
+  return PixTile{(mt - ty * G.conv_xt) * G.conv_bx, ty * G.conv_by};
 }
 
 __device__ __forceinline__ float2 ld_bf16x2(const bf16* p) {
@@ -271,7 +272,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
         const PixTile pt = pix_tile(G, tc.m0);
         const int x = pt.x0 + rl % G.conv_bx, y = pt.y0 + rl / G.conv_bx;
         orow[h2] = (y + 1) * (G.conv_w + 2) + x + 1;
-        ok[h2] = true;
+        ok[h2] = x < G.conv_w && y < G.conv_h;  // a ragged tile's pixels past the image: the ring stays zero
       } else {
         orow[h2] = tc.m0 + rl;
         ok[h2] = orow[h2] < G.M;
@@ -678,18 +679,37 @@ int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT
 // ring: in [(Hin+2)(Win+2), Cin], out [(H+2)(W+2), Cout] (interior written, ring untouched), weights
 // [Cout, taps * Cin] (tap-major K), optional residual res (same geometry as out) added after the bias
 // rounding (ResnetBlock2D: x + conv2(...)).  H, W are the OUTPUT size; Hin = stride * H.
-// Needs: Cin % 64 == 0, Cout % 128 == 0, W a power of two >= 8 (or a multiple of 128), H % (128/bx) == 0.
+// Needs: Cin % 64 == 0, Cout % 128 == 0, H, W >= 1.
+
+// Pixel tile width bx (a power of two in [8, 128]; by = 128 / bx rows) of an H x W output: the one whose
+// ceil(W / bx) x ceil(H / by) tiles cover the least area, the widest of equals.  Every tile computes all
+// 128 pixels, so the area past the image is wasted MMA work: 96 x 168 fits exactly with bx = 8, where bx = 128
+// would waste 34 %.  The geometries that fit exactly at bx = min(W, 128) keep that width.
+int conv_tile_width(int H, int W) {
+  int best = 128;
+  long long best_area = -1;
+  for (int bx = 128; bx >= 8; bx /= 2) {
+    const int by = 128 / bx;
+    const long long area = static_cast<long long>((W + bx - 1) / bx) * ((H + by - 1) / by);
+    if (best_area < 0 || area < best_area) {
+      best = bx;
+      best_area = area;
+    }
+  }
+  return best;
+}
+
 int conv_launch(const bf16* in, const bf16* weight, const bf16* bias, bf16* out, const bf16* res,
                 const bf16* ones, int H, int W, int Cin, int Cout, int taps, int stride,
                 cudaStream_t stream) {
-  const int bx = W >= 128 ? 128 : W;
-  const int by = 128 / bx;
   if (Cin % 64 != 0 || Cout % 128 != 0 || (taps != 9 && taps != 1) || (stride != 1 && stride != 2) ||
-      W % bx != 0 || 128 % bx != 0 || H % by != 0) {
-    set_error("conv_launch: unsupported geometry (Cin % 64, Cout % 128, W = 2^k or multiple of 128, "
-              "H divisible by 128 / min(W, 128))");
+      H < 1 || W < 1) {
+    set_error("conv_launch: unsupported geometry (Cin % 64, Cout % 128, 1x1 or 3x3, stride 1 or 2)");
     return -1;
   }
+  const int bx = conv_tile_width(H, W);
+  const int by = 128 / bx;
+  const int xt = (W + bx - 1) / bx, yt = (H + by - 1) / by;
   const int bn = (Cout % 256 == 0) ? 256 : 128;
   GemmParamsDev p;
   memset(&p, 0, sizeof(p));
@@ -712,8 +732,10 @@ int conv_launch(const bf16* in, const bf16* weight, const bf16* bias, bf16* out,
   d.ldr = Cout;
   d.gate = ones;  // residual epilogue = bf16(res + bf16(1 * y))
   d.M = H * W;
-  d.m_tiles = d.M / BM;
+  d.m_tiles = xt * yt;
   d.conv_w = W;
+  d.conv_h = H;
+  d.conv_xt = xt;
   d.conv_taps = taps;
   d.conv_cin_blocks = Cin / BK;
   d.conv_bx = bx;

@@ -211,17 +211,29 @@ __global__ void repad_kernel(const bf16* __restrict__ x, bf16* __restrict__ out,
     *(reinterpret_cast<uint4*>(out + orow * C) + o) = __ldg(reinterpret_cast<const uint4*>(x + irow * C) + o);
   }
 }
-// in-place row softmax of a bf16 score matrix: p = softmax(s * scale) (fp32 math, bf16 out)
+// in-place row softmax of a bf16 score matrix: p = softmax(s * scale) (fp32 math, bf16 out).  Rows have n
+// columns (n % 8 == 0); the keys [valid, n) are padding: probability 0, outside the max and the row sum.
 __global__ void __launch_bounds__(256)
-softmax_rows_kernel(bf16* __restrict__ s, int n, float scale) {
+softmax_rows_kernel(bf16* __restrict__ s, int n, int valid, float scale) {
   __shared__ float red[8];
   bf16* row = s + static_cast<size_t>(blockIdx.x) * n;
   const float sl = scale * 1.4426950408889634f;
+  // padded columns read as -inf: exp2(-inf) = 0 leaves the max and the sum exactly as without them
+  auto load = [&](int i, float (&v)[8]) {
+    const uint4 u = *reinterpret_cast<const uint4*>(row + i);
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float2 f = unpack_bf16x2(w[q]);
+      v[2 * q] = i + 2 * q < valid ? f.x : -INFINITY;
+      v[2 * q + 1] = i + 2 * q + 1 < valid ? f.y : -INFINITY;
+    }
+  };
   float mx = -INFINITY;
   for (int i = threadIdx.x * 8; i < n; i += blockDim.x * 8) {
-    const uint4 u = *reinterpret_cast<const uint4*>(row + i);
-    const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-    mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(b.x, b.y)), fmaxf(fmaxf(c.x, c.y), fmaxf(d.x, d.y))));
+    float v[8];
+    load(i, v);
+    mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(v[0], v[1]), fmaxf(v[2], v[3])), fmaxf(fmaxf(v[4], v[5]), fmaxf(v[6], v[7]))));
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
@@ -233,13 +245,10 @@ softmax_rows_kernel(bf16* __restrict__ s, int n, float scale) {
   __syncthreads();
   float sum = 0.f;
   for (int i = threadIdx.x * 8; i < n; i += blockDim.x * 8) {
-    const uint4 u = *reinterpret_cast<const uint4*>(row + i);
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    float v[8];
+    load(i, v);
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 v = unpack_bf16x2(w[q]);
-      sum += exp2f((v.x - mx) * sl) + exp2f((v.y - mx) * sl);
-    }
+    for (int q = 0; q < 4; ++q) sum += exp2f((v[2 * q] - mx) * sl) + exp2f((v[2 * q + 1] - mx) * sl);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -250,14 +259,12 @@ softmax_rows_kernel(bf16* __restrict__ s, int n, float scale) {
   for (int i = 0; i < 8; ++i) sum += red[i];
   const float inv = 1.0f / sum;
   for (int i = threadIdx.x * 8; i < n; i += blockDim.x * 8) {
-    const uint4 u = *reinterpret_cast<const uint4*>(row + i);
-    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    float v[8];
+    load(i, v);
     uint32_t o[4];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 v = unpack_bf16x2(w[q]);
-      o[q] = pack_bf16x2(exp2f((v.x - mx) * sl) * inv, exp2f((v.y - mx) * sl) * inv);
-    }
+    for (int q = 0; q < 4; ++q)
+      o[q] = pack_bf16x2(exp2f((v[2 * q] - mx) * sl) * inv, exp2f((v[2 * q + 1] - mx) * sl) * inv);
     *reinterpret_cast<uint4*>(row + i) = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
@@ -482,6 +489,8 @@ int make_mid(rf_vae* h, MidBlock& m, const std::string& key) {
 }
 
 size_t padded_elems(int H, int W, int C) { return static_cast<size_t>(H + 2) * (W + 2) * C; }
+// keys of the mid-block attention, padded to whole 128-row tiles (the S GEMM's N, the PV GEMM's K)
+int padded_tokens(int H, int W) { return (H * W + 127) / 128 * 128; }
 
 int grid_for(long long work, int threads = 256) {
   long long b = (work + threads - 1) / threads;
@@ -527,9 +536,39 @@ void drop_graphs(rf_vae* h) {
   h->graphs.clear();
 }
 
+void vfree(rf_vae* h, void* p) {
+  if (!p) return;
+  for (size_t i = 0; i < h->allocs.size(); ++i)
+    if (h->allocs[i] == p) {
+      h->allocs.erase(h->allocs.begin() + i);
+      break;
+    }
+  cudaFree(p);
+}
+
+// Every workspace size grows with the image height and width, so a workspace for (ws_h, ws_w) serves any
+// image that fits inside both.  A larger request grows it to the larger of each side (a 1024x1024 call after a
+// 768x1344 one makes room for 1024x1344), so alternating shapes allocate once, and frees the old one.
 int ensure_workspace(rf_vae* h, int H, int W) {  // H, W: output image size
   if (h->ws_h >= H && h->ws_w >= W && h->buf[0]) return 0;
   drop_graphs(h);  // they reference the old workspace
+  if (H < h->ws_h) H = h->ws_h;
+  if (W < h->ws_w) W = h->ws_w;
+  if (h->buf[0]) RF_CHECK_CUDA(cudaDeviceSynchronize());  // work still queued on the old buffers
+  void** old[] = {reinterpret_cast<void**>(&h->g_u8), reinterpret_cast<void**>(&h->g_chw),
+                  reinterpret_cast<void**>(&h->g_lat), reinterpret_cast<void**>(&h->g_eps),
+                  reinterpret_cast<void**>(&h->buf[0]), reinterpret_cast<void**>(&h->buf[1]),
+                  reinterpret_cast<void**>(&h->buf[2]), reinterpret_cast<void**>(&h->buf[3]),
+                  reinterpret_cast<void**>(&h->tok), reinterpret_cast<void**>(&h->tokx),
+                  reinterpret_cast<void**>(&h->qkv), reinterpret_cast<void**>(&h->S),
+                  reinterpret_cast<void**>(&h->vt), reinterpret_cast<void**>(&h->ao),
+                  reinterpret_cast<void**>(&h->ay)};
+  for (void** q : old) {
+    vfree(h, *q);
+    *q = nullptr;
+  }
+  h->ws_h = h->ws_w = 0;  // stays 0 if an allocation below fails: the next call starts over
+  for (int i = 0; i < 4; ++i) h->tag[i] = -1;
   const int lh = H / 8, lw = W / 8;
   {
     void* q;
@@ -545,14 +584,16 @@ int ensure_workspace(rf_vae* h, int H, int W) {  // H, W: output image size
     RF_TRYV(valloc(h, &p, big * 2));
     h->buf[i] = static_cast<bf16*>(p);
   }
-  const size_t ntok = static_cast<size_t>(lh) * lw;
+  // mid-block attention (decoder at H/8 x W/8; the encoder's is the same size): qkv, the staged K (ay) and V^T
+  // run to the padded key count
+  const size_t ntok = static_cast<size_t>(lh) * lw, npad = padded_tokens(lh, lw);
   RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->tok = static_cast<bf16*>(p);
   RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->tokx = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * 1536 * 2)); h->qkv = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * ntok * 2)); h->S = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->vt = static_cast<bf16*>(p);
+  RF_TRYV(valloc(h, &p, npad * 1536 * 2)); h->qkv = static_cast<bf16*>(p);
+  RF_TRYV(valloc(h, &p, ntok * npad * 2)); h->S = static_cast<bf16*>(p);
+  RF_TRYV(valloc(h, &p, npad * 512 * 2)); h->vt = static_cast<bf16*>(p);
   RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->ao = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->ay = static_cast<bf16*>(p);
+  RF_TRYV(valloc(h, &p, npad * 512 * 2)); h->ay = static_cast<bf16*>(p);
   if (!h->gn_acc) {
     RF_TRYV(valloc(h, &p, sizeof(float) * 2 * 128 * rf::kGnBlocks)); h->gn_acc = static_cast<float*>(p);
     RF_TRYV(valloc(h, &p, sizeof(float) * 64)); h->gn_mr = static_cast<float*>(p);
@@ -590,10 +631,12 @@ int resnet(rf_vae* h, const Resnet& r, int x, int out, int t1, int t2, int H, in
 }
 
 // UNetMidBlock2D: resnet, self-attention over H*W tokens (1 head x 512), resnet.  buf[x] -> buf[x].
+// The keys run to npad = padded_tokens(H, W): K / V rows [ntok, npad) are zero and the softmax gives them
+// probability 0, so the padding changes no result.  With ntok % 128 == 0 there is no padding.
 int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int H, int W, cudaStream_t s) {
   RF_TRYV(resnet(h, m.res[0], x, y, t1, t2, H, W, s));
   std::swap(x, y);
-  const int ntok = H * W;
+  const int ntok = H * W, npad = padded_tokens(H, W);
   RF_TRYV(group_norm(h, h->buf[x], h->tok, H, W, m.attn_gn, 0, 1, 0, s));  // compact tokens
   rf::repad_kernel<<<grid_for(static_cast<long long>(ntok) * 64), 256, 0, s>>>(h->buf[x], h->tokx, H, W, 512,
                                                                               1, 0);
@@ -604,25 +647,29 @@ int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int 
   g.A = h->tok; g.lda = 512; g.M = ntok; g.W = m.attn_qkv.w; g.bias = m.attn_qkv.b;
   g.out = h->qkv; g.ldo = 1536;
   RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 1536, 512, 1, &g, s));
+  // q | k | v rows of the padding keys (the GEMM writes rows [0, ntok) only)
+  if (npad > ntok)
+    RF_CHECK_CUDA(cudaMemsetAsync(h->qkv + static_cast<size_t>(ntok) * 1536, 0,
+                                  static_cast<size_t>(npad - ntok) * 1536 * 2, s));
   // the GEMM's W operand is [N, K] with pitch K: stage K compactly (ay is free until the out-proj)
-  RF_CHECK_CUDA(cudaMemcpy2DAsync(h->ay, 512 * 2, h->qkv + 512, 1536 * 2, 512 * 2, ntok,
+  RF_CHECK_CUDA(cudaMemcpy2DAsync(h->ay, 512 * 2, h->qkv + 512, 1536 * 2, 512 * 2, npad,
                                   cudaMemcpyDeviceToDevice, s));
-  memset(&g, 0, sizeof(g));  // S = Q K^T
-  g.A = h->qkv; g.lda = 1536; g.M = ntok; g.W = h->ay; g.out = h->S; g.ldo = ntok;
-  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, ntok, 512, 1, &g, s));
+  memset(&g, 0, sizeof(g));  // S = Q K^T  [ntok, npad]
+  g.A = h->qkv; g.lda = 1536; g.M = ntok; g.W = h->ay; g.out = h->S; g.ldo = npad;
+  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, npad, 512, 1, &g, s));
   {
-    rf::ProfScope prof("vae_softmax", 0, 4.0 * ntok * ntok, s);
-    rf::softmax_rows_kernel<<<ntok, 256, 0, s>>>(h->S, ntok, 1.0f / sqrtf(512.0f));
+    rf::ProfScope prof("vae_softmax", 0, 4.0 * ntok * npad, s);
+    rf::softmax_rows_kernel<<<ntok, 256, 0, s>>>(h->S, npad, ntok, 1.0f / sqrtf(512.0f));
   }
   RF_CHECK_CUDA(cudaGetLastError());
   rf::count_launch();
-  dim3 tg(512 / 32, ntok / 32), tb(32, 8);
-  rf::transpose_kernel<<<tg, tb, 0, s>>>(h->qkv + 1024, 1536, h->vt, ntok, 512);  // V^T [512, ntok]
+  dim3 tg(512 / 32, npad / 32), tb(32, 8);
+  rf::transpose_kernel<<<tg, tb, 0, s>>>(h->qkv + 1024, 1536, h->vt, npad, 512);  // V^T [512, npad]
   RF_CHECK_CUDA(cudaGetLastError());
   rf::count_launch();
   memset(&g, 0, sizeof(g));  // O = P V
-  g.A = h->S; g.lda = ntok; g.M = ntok; g.W = h->vt; g.out = h->ao; g.ldo = 512;
-  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 512, ntok, 1, &g, s));
+  g.A = h->S; g.lda = npad; g.M = ntok; g.W = h->vt; g.out = h->ao; g.ldo = 512;
+  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 512, npad, 1, &g, s));
   memset(&g, 0, sizeof(g));  // y = x + to_out(O)
   g.A = h->ao; g.lda = 512; g.M = ntok; g.W = m.attn_out.w; g.bias = m.attn_out.b;
   g.out = h->ay; g.ldo = 512; g.res = h->tokx; g.ldr = 512; g.gate = h->ones;
@@ -635,6 +682,18 @@ int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int 
   std::swap(x, y);
   RF_TRYV(resnet(h, m.res[1], x, y, t1, t2, H, W, s));
   std::swap(x, y);
+  return 0;
+}
+
+// Any image whose sides are multiples of 16 (one latent token = 16 x 16 pixels), as diffusers' FLUX pipeline
+// accepts.  The cap keeps pixel indices in 32 bits; well below it the workspace (the mid-block's
+// (H/8 * W/8)^2 score matrix) outgrows the device, and ensure_workspace reports the failed allocation.
+int check_size(const char* fn, int height, int width) {
+  if (height % 16 != 0 || width % 16 != 0 || height < 16 || width < 16 || height > 16384 || width > 16384) {
+    rf::set_error(std::string(fn) + ": height and width must be multiples of 16 in [16, 16384], got " +
+                  std::to_string(height) + "x" + std::to_string(width));
+    return -1;
+  }
   return 0;
 }
 
@@ -846,16 +905,7 @@ int rf_vae_decode(rf_vae* h, const void* packed_latents, int height, int width, 
     rf::set_error("rf_vae_decode: null argument");
     return -1;
   }
-  {
-    const int lw = width / 8, lh = height / 8;
-    const int bx = lw >= 128 ? 128 : lw;
-    if (height % 16 != 0 || width % 16 != 0 || lw < 8 || lw % bx != 0 || 128 % bx != 0 ||
-        lh % (128 / bx) != 0 || (lh * lw) % 256 != 0) {
-      rf::set_error("rf_vae_decode: height, width must be multiples of 16 with width/8 a power of two "
-                    "(or a multiple of 128) and (height/8)*(width/8) a multiple of 256");
-      return -1;
-    }
-  }
+  RF_TRYV(check_size("rf_vae_decode", height, width));
   RF_TRYV(ensure_workspace(h, height, width));
   if (vae_missing(h, "decoder.") != 0) return -4;
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
@@ -939,16 +989,7 @@ int rf_vae_encode(rf_vae* h, const uint8_t* image_u8_hwc, const void* image_bf16
     rf::set_error("rf_vae_encode: null argument");
     return -1;
   }
-  {
-    const int lw = width / 8, lh = height / 8;
-    const int bx = lw >= 128 ? 128 : lw;
-    if (height % 16 != 0 || width % 16 != 0 || lw < 8 || lw % bx != 0 || 128 % bx != 0 ||
-        lh % (128 / bx) != 0 || (lh * lw) % 256 != 0) {
-      rf::set_error("rf_vae_encode: height, width must be multiples of 16 with width/8 a power of two "
-                    "(or a multiple of 128) and (height/8)*(width/8) a multiple of 256");
-      return -1;
-    }
-  }
+  RF_TRYV(check_size("rf_vae_encode", height, width));
   RF_TRYV(ensure_workspace(h, height, width));
   if (vae_missing(h, "encoder.") != 0) return -4;
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
