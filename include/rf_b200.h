@@ -123,7 +123,7 @@ typedef struct rf_dit_config {
   int joint_attention_dim; /* 4096 (T5 width)                       */
   int pooled_projection_dim; /* 768 (CLIP pooled width)             */
   int guidance_embeds;     /* 1 for FLUX.1-dev                      */
-  int lora_rank;           /* 0 = no LoRA storage; else rank (<= 64) of the condition LoRA */
+  int lora_rank;           /* 0 = no LoRA storage; else max rank (<= 64) of the LoRA (cond tokens, + latent_lora) */
 } rf_dit_config;
 
 int rf_dit_create(const rf_dit_config* cfg, rf_dit** out);
@@ -140,7 +140,9 @@ int rf_dit_load_weight(rf_dit* h, const char* key, const void* src, int64_t nume
  * (e.g. "single_transformer_blocks.0.proj_out"); A: [r, in_features] bf16, B: [out_features, r]
  * bf16 (device); in_/out_features are checked against the target Linear (a mismatched adapter
  * file is an error, not an out-of-bounds read); scale = lora_alpha / r.  Applied to condition
- * tokens only unless latent_lora is set in rf_dit_prepare (lora_controller.py:5-42). */
+ * tokens only unless latent_lora is set in rf_dit_prepare (lora_controller.py:5-42); with it, to every
+ * token that passes the target: the image stream of the double blocks, the txt + img rows of the single
+ * blocks, and the image / main-row adaLN modulation (norm1.linear / norm.linear of temb). */
 int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B, int r,
                     int in_features, int out_features, float scale);
 
@@ -151,9 +153,10 @@ int rf_dit_missing_weights(rf_dit* h);
  * Builds the RoPE tables once (the reference rebuilds them every step, transformer.py:130-134)
  * and sizes the workspace.  n_cond = 0 selects entry A (stock FluxTransformer2DModel.forward);
  * n_cond > 0 selects entry B (train_flux/flux/transformer.py:47 tranformer_forward).
- * flags: bit0 latent_lora, bit1 add_cond_attn, bit2 union_cond_attn==False, bit3 = apply the LoRA
- * as merged weights W + B A for the condition tokens (peft fuse_lora semantics: one rounding of
- * the merged weight instead of three roundings of the low-rank path; no extra launches);
+ * flags: bit0 latent_lora (LoRA on the image and text tokens too; entry A included), bit1
+ * add_cond_attn (not implemented: fails), bit2 union_cond_attn==False, bit3 = apply the LoRA as merged
+ * weights W + B A for the LoRA'd tokens (peft fuse_lora semantics: one rounding of the merged weight
+ * instead of three roundings of the low-rank path; no extra launches; adaLN terms stay unfused);
  * condition_scale != 1 enables the c_factor attention bias (generate.py:86-90). */
 int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const void* txt_ids,
                    const void* img_ids, const void* cond_ids, int flags, float condition_scale,

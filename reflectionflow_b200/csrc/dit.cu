@@ -5,7 +5,8 @@
 //   train_flux/flux/transformer.py:47-252 (tranformer_forward; with n_cond == 0 the stock
 //   diffusers FluxTransformer2DModel.forward), train_flux/flux/block.py:173-333 (block_forward,
 //   single_block_forward, attn_forward), train_flux/flux/generate.py:217-276 (denoise loop),
-//   train_flux/flux/lora_controller.py:5-42 (LoRA on condition tokens only).
+//   train_flux/flux/lora_controller.py:5-42 (LoRA on condition tokens only; with latent_lora on every token
+//   that passes a target Linear).
 //
 // HBM layout (token-major, one joint buffer per quantity; rows = [txt | img | cond]):
 //   X   [N, D]      hidden state (residual stream), updated in place by the GEMM epilogues
@@ -111,7 +112,8 @@ struct rf_dit {
   float *rope_cos = nullptr, *rope_sin = nullptr, *crope_cos = nullptr, *crope_sin = nullptr;
   // ---- workspace
   bf16 *X = nullptr, *XN = nullptr, *QKV = nullptr, *ACT = nullptr, *MOD = nullptr, *MODC = nullptr;
-  bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [rows, 192], L [rows, 4D]
+  bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [lora_rows, 256], L [lora_rows, 4D]
+  int lora_rows = 0;
   bf16 *emb_tmp = nullptr;            // small vectors for the temb path
   bf16 *temb = nullptr, *ctemb = nullptr;
   // ---- staging for the graph-captured denoise loop
@@ -322,35 +324,43 @@ int compute_temb(rf_dit* h, const bf16* t, const int* step, const bf16* guid, co
   return 0;
 }
 
-// L[rows, out] = bf16( bf16(x A^T) B^T ): the peft low-rank term for `rows` condition tokens
-int lora_term(rf_dit* h, const LoraT& t, const bf16* x, int ldx, int rows, bf16* L, int ldl,
-              cudaStream_t s) {
-  rf::GemmGroupArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = x; g.lda = ldx; g.M = rows; g.W = t.A; g.out = h->LT; g.ldo = kLoraPad;
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, kLoraPad, t.in, 1, &g, s));
-  memset(&g, 0, sizeof(g));
-  g.A = h->LT; g.lda = kLoraPad; g.M = rows; g.W = t.B; g.out = L; g.ldo = ldl;
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, t.out, kLoraPad, 1, &g, s));
-  return 0;
+// L[rows, :] = bf16( bf16(x A^T) B^T ): the unfused peft low-rank term of `rows` tokens for n = 1 target, or for
+// the n = 3 stacked q|k|v targets (A_all = [Aq;Ak;Av]: T = x A_all^T in one GEMM, L[:, jD:(j+1)D] = T_j B_j^T
+// grouped).  T != nullptr: bf16(x A_all^T) of these rows was already computed (pitch ld_t); only the up-projection
+// runs.  Otherwise T is computed here into LT.
+int lora_term(rf_dit* h, const LoraT* const* ls, int n, const bf16* A_all, const bf16* x, int ldx, int rows,
+              const bf16* T, int ld_t, bf16* L, int ldl, cudaStream_t s) {
+  rf::GemmGroupArgs g[3];
+  if (T == nullptr) {
+    memset(g, 0, sizeof(g));
+    g[0].A = x; g[0].lda = ldx; g[0].M = rows; g[0].W = A_all; g[0].out = h->LT; g[0].ldo = n * kLoraPad;
+    RF_TRY(rf::gemm_launch(rf::EPI_BIAS, n * kLoraPad, ls[0]->in, 1, g, s));
+    T = h->LT;
+    ld_t = n * kLoraPad;
+  }
+  memset(g, 0, sizeof(g));
+  for (int j = 0; j < n; ++j) {
+    g[j].A = T + j * kLoraPad; g[j].lda = ld_t; g[j].M = rows;
+    g[j].W = ls[j]->B; g[j].out = L + static_cast<int64_t>(j) * ls[j]->out; g[j].ldo = ldl;
+  }
+  return rf::gemm_launch(rf::EPI_BIAS, ls[0]->out, kLoraPad, n, g, s);
 }
 
-// fused q|k|v low-rank term: T = x [Aq;Ak;Av]^T (one GEMM), L[:, jD:(j+1)D] = T_j B_j^T (grouped)
-int lora_term_qkv(rf_dit* h, const bf16* qkvA, const LoraT& lq, const LoraT& lk, const LoraT& lv,
-                  const bf16* x, int ldx, int rows, bf16* L, int ldl, cudaStream_t s) {
+// The low-rank term of the adaLN Linears (norm1.linear of the double blocks, norm.linear of the single blocks)
+// added to their sections of `batch` modulation rows: mod[b * ld_mod + section] += bf16(bf16(silu(emb_b) A^T) B^T)
+// (peft: bf16(y + L)).  M = batch is tiny: two batched GEMVs and one strided add per target.
+// tvec: [batch, 64], lvec: [batch, 6D] scratch.
+int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bf16* mod, int64_t ld_mod, bf16* tvec, bf16* lvec,
+                 cudaStream_t s) {
   const int D = h->D;
-  rf::GemmGroupArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = x; g.lda = ldx; g.M = rows; g.W = qkvA; g.out = h->LT; g.ldo = 3 * kLoraPad;
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, 3 * kLoraPad, D, 1, &g, s));
-  rf::GemmGroupArgs gg[3];
-  memset(gg, 0, sizeof(gg));
-  const LoraT* ls[3] = {&lq, &lk, &lv};
-  for (int j = 0; j < 3; ++j) {
-    gg[j].A = h->LT + j * kLoraPad; gg[j].lda = 3 * kLoraPad; gg[j].M = rows;
-    gg[j].W = ls[j]->B; gg[j].out = L + static_cast<int64_t>(j) * D; gg[j].ldo = ldl;
-  }
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, D, kLoraPad, 3, gg, s));
+  auto one = [&](const LoraT& t, int64_t off) -> int {
+    if (!t.set) return 0;
+    RF_TRY(rf::gemv_launch(emb, D, batch, t.A, nullptr, tvec, kLoraPad, kLoraPad, D, 1, s));
+    RF_TRY(rf::gemv_launch(tvec, kLoraPad, batch, t.B, nullptr, lvec, t.out, t.out, kLoraPad, 0, s));
+    return rf::add_rows_launch(mod + off, ld_mod, lvec, t.out, batch, t.out, s);
+  };
+  for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1, mod_double(h, i, 0, 0)));
+  for (int i = 0; i < h->cfg.num_single_layers; ++i) RF_TRY(one(h->sgl[i].l_norm, mod_single(h, i, 0)));
   return 0;
 }
 
@@ -362,26 +372,8 @@ int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
   RF_TRY(rf::gemv_launch(h->ctemb, D, 1, h->modW, h->modB, h->MODC, static_cast<int>(h->n_mod),
                          static_cast<int>(h->n_mod), D, 1, s));
   if (!h->any_lora) return 0;
-  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb): M = 1 -> two GEMVs + add
-  bf16* tvec = h->LT;          // [64]
-  bf16* lvec = h->LT + 256;    // [6D]
-  for (int i = 0; i < h->cfg.num_layers; ++i) {
-    const LoraT& t = h->dbl[i].l_norm1;
-    if (!t.set) continue;
-    bf16* dst = h->MODC + mod_double(h, i, 0, 0);
-    RF_TRY(rf::gemv_launch(h->ctemb, D, 1, t.A, nullptr, tvec, kLoraPad, kLoraPad, D, 1, s));
-    RF_TRY(rf::gemv_launch(tvec, kLoraPad, 1, t.B, nullptr, lvec, 6 * D, 6 * D, kLoraPad, 0, s));
-    RF_TRY(rf::add2_launch(dst, lvec, dst, 6 * D, s));
-  }
-  for (int i = 0; i < h->cfg.num_single_layers; ++i) {
-    const LoraT& t = h->sgl[i].l_norm;
-    if (!t.set) continue;
-    bf16* dst = h->MODC + mod_single(h, i, 0);
-    RF_TRY(rf::gemv_launch(h->ctemb, D, 1, t.A, nullptr, tvec, kLoraPad, kLoraPad, D, 1, s));
-    RF_TRY(rf::gemv_launch(tvec, kLoraPad, 1, t.B, nullptr, lvec, 3 * D, 3 * D, kLoraPad, 0, s));
-    RF_TRY(rf::add2_launch(dst, lvec, dst, 3 * D, s));
-  }
-  return 0;
+  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb)
+  return add_mod_lora(h, h->ctemb, 1, h->MODC, h->n_mod, h->LT, h->LT + 256, s);
 }
 
 // fuse_lora mode: merged weights for the condition-token groups (allocated on first use)
@@ -429,7 +421,8 @@ int merge_all(rf_dit* h, cudaStream_t s) {
 int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16* guid,
                          const bf16* pooled, cudaStream_t s) {
   const int D = h->D;
-  bf16* ws = h->s_temb_ws;  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c
+  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c | [n,64] | [n,6D] (LoRA)
+  bf16* ws = h->s_temb_ws;
   bf16* tp = ws;
   bf16* tmp = tp + static_cast<int64_t>(n_steps) * 256;
   bf16* a = tmp + static_cast<int64_t>(n_steps) * D;
@@ -452,6 +445,13 @@ int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16*
   }
   RF_TRY(rf::gemv_launch(temb, D, n_steps, h->modW, h->modB, h->s_mod_all, static_cast<int>(h->n_mod),
                          static_cast<int>(h->n_mod), D, 1, s));
+  // latent_lora: the adaLN LoRA of the image stream (double blocks) / of the txt+img rows (single blocks) acts on
+  // silu(temb_i), which every step knows before the loop: its term joins the table here too
+  if ((h->flags & 1) && h->any_lora) {
+    bf16* tvec = c + D;                                      // [n, 64]
+    bf16* lvec = tvec + static_cast<int64_t>(n_steps) * kLoraPad;  // [n, 6D]
+    RF_TRY(add_mod_lora(h, temb, n_steps, h->s_mod_all, h->n_mod, tvec, lvec, s));
+  }
   return 0;
 }
 
@@ -465,6 +465,9 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
                     bf16* out, cudaStream_t s, const bf16* mod_all = nullptr) {
   const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D;
   const bool use_cond = h->n_cond > 0;
+  // latent_lora (lora_controller.py:5-9): the LoRA also acts on the image stream of the double blocks and on the
+  // txt + img rows of the single blocks (the text stream of the double blocks has no LoRA target)
+  const bool ll = (h->flags & 1) != 0;
   const StreamRows S_txt{0, h->n_txt}, S_img{h->n_txt, h->n_img}, S_cond{h->n_main, h->n_cond};
   bf16 *X = h->X, *XN = h->XN, *QKV = h->QKV, *ACT = h->ACT;
   auto rowp = [&](bf16* base, int ld, int row) { return base + static_cast<int64_t>(row) * ld; };
@@ -478,13 +481,21 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   if (use_cond) {
     g[1] = g[0];
     g[1].A = cond_lat; g[1].M = h->n_cond; g[1].out = rowp(X, D, S_cond.row0);
-    if (h->use_merged) {
-      g[1].W = h->x_emb_m;
-    } else if (h->l_x_emb.set) {
-      RF_TRY(lora_term(h, h->l_x_emb, cond_lat, h->cfg.in_channels, h->n_cond, h->LL, D, s));
-      g[1].addend = h->LL; g[1].ldadd = D;
-    }
     ng = 2;
+  }
+  if (h->use_merged) {
+    if (ll) g[0].W = h->x_emb_m;
+    if (use_cond) g[1].W = h->x_emb_m;
+  } else if (h->l_x_emb.set) {
+    // K = 64, EPI_BIAS: the unfused low-rank term, each LoRA'd group's L in its own rows of LL
+    const LoraT* xl = &h->l_x_emb;
+    int row = 0;
+    for (int j = ll ? 0 : 1; j < ng; ++j) {
+      bf16* L = rowp(h->LL, D, row);
+      RF_TRY(lora_term(h, &xl, 1, xl->A, g[j].A, g[j].lda, g[j].M, nullptr, 0, L, D, s));
+      g[j].addend = L; g[j].ldadd = D;
+      row += g[j].M;
+    }
   }
   RF_TRY(rf::gemm_launch(rf::EPI_BIAS, D, h->cfg.in_channels, ng, g, s));
   memset(g, 0, sizeof(g));
@@ -499,6 +510,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     RF_TRY(compute_temb(h, tstep, step_idx, guid, pooled, h->temb, s));
     RF_TRY(rf::gemv_launch(h->temb, D, 1, h->modW, h->modB, h->MOD, static_cast<int>(h->n_mod),
                            static_cast<int>(h->n_mod), D, 1, s));
+    if (ll && h->any_lora) RF_TRY(add_mod_lora(h, h->temb, 1, h->MOD, h->n_mod, h->LT, h->LT + 256, s));
   }
   const bf16* MOD = h->MOD;
   const bf16* MODC = h->MODC;
@@ -507,24 +519,57 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     return rf::ln_modulate_launch(rowp(X, D, sr.row0), D, rowp(XN, D, sr.row0), D, sr.rows, D, scale,
                                   shift, sr.rows, 0, s);
   };
-  // A grouped GEMM whose LAST group is the condition stream carrying a LoRA (exact mode).  Fast path:
-  // T = bf16(x A^T) (one skinny GEMM), then ONE grouped launch of all streams in which the condition
-  // stream's tiles carry the low-rank k-block (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Small /
-  // odd shapes keep the unfused path: L materialised by two GEMMs and added in the epilogue (`addend`).
-  // (t_pre != nullptr: T was already produced by an earlier launch, [M, ld_t] with this target's columns at t_pre)
-  auto gemm_cond_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const bf16* loraA,
-                            int t_cols, const bf16* loraB, int sec_cols, auto&& unfused_term,
-                            const bf16* t_pre = nullptr, int ld_t = 0) -> int {
-    rf::GemmGroupArgs& gc = gr[ngr - 1];
-    if (rf::gemm_lora_eligible(epi, N, K, gc)) {
-      if (t_pre == nullptr) {
-        RF_TRY(rf::lora_down_launch(gc.A, gc.lda, gc.M, K, loraA, t_cols, h->LT, t_cols, s));
-        t_pre = h->LT;
-        ld_t = t_cols;
+  // The groups of a projection launch that carry the LoRA in exact mode, in row order: the image (double blocks) or
+  // txt + img (single blocks) group under latent_lora, then the condition group.  Their rows are contiguous in the
+  // joint buffers ([n_txt, N) resp. [0, N)), so one down-projection over that range serves all of them; `row` is
+  // each group's first row inside the range, i.e. its row in LT / LL.
+  struct LoraGroups {
+    int n = 0, rows = 0;
+    int idx[2] = {0, 0};
+    int row[2] = {0, 0};
+    void add(int i, int m) { idx[n] = i; row[n] = rows; rows += m; ++n; }
+  };
+  auto lora_groups = [&](bool target_set, int main_idx, int main_rows, int cond_idx) {
+    LoraGroups lg;
+    if (!target_set || h->use_merged) return lg;
+    if (ll) lg.add(main_idx, main_rows);
+    if (use_cond) lg.add(cond_idx, h->n_cond);
+    return lg;
+  };
+  // merged mode (fuse_lora): the same groups read the merged weights W + B A instead
+  auto merged_w = [&](rf::GemmGroupArgs* gr, int main_idx, int cond_idx, const bf16* Wm) {
+    if (!h->use_merged) return;
+    if (ll) gr[main_idx].W = Wm;
+    if (use_cond) gr[cond_idx].W = Wm;
+  };
+  // A grouped GEMM in which the groups `lg` carry the LoRA of `ls` (one target, or the three stacked q|k|v
+  // targets; A_all / B_all their stacked factors).  Fast path: T = bf16(x A^T) for all LoRA'd rows (one skinny
+  // GEMM), then ONE grouped launch of all streams in which the eligible groups' tiles carry the low-rank k-block
+  // (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Groups too small for it (gemm_lora_eligible) keep the
+  // unfused path: L materialised in their rows of LL and added in the epilogue (`addend`); they reuse T when it
+  // exists.  (t_pre != nullptr: T was already produced by an earlier launch, [rows, ld_t] with this target's
+  // columns at t_pre.)
+  auto gemm_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const LoraGroups& lg,
+                       const LoraT* const* ls, int nls, const bf16* A_all, const bf16* B_all, int ldl,
+                       const bf16* t_pre = nullptr, int ld_t = 0) -> int {
+    bool fused[2] = {false, false}, any_fused = false;
+    for (int j = 0; j < lg.n; ++j) any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, gr[lg.idx[j]]));
+    if (any_fused && t_pre == nullptr) {
+      const rf::GemmGroupArgs& g0 = gr[lg.idx[0]];
+      RF_TRY(rf::lora_down_launch(g0.A, g0.lda, lg.rows, K, A_all, nls * kLoraPad, h->LT, nls * kLoraPad, s));
+      t_pre = h->LT;
+      ld_t = nls * kLoraPad;
+    }
+    for (int j = 0; j < lg.n; ++j) {
+      rf::GemmGroupArgs& gc = gr[lg.idx[j]];
+      const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(lg.row[j]) * ld_t : nullptr;
+      if (fused[j]) {
+        gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = B_all; gc.lora_sec_cols = nls > 1 ? ls[0]->out : 0;
+      } else {
+        bf16* L = rowp(h->LL, ldl, lg.row[j]);
+        RF_TRY(lora_term(h, ls, nls, A_all, gc.A, gc.lda, gc.M, t_rows, ld_t, L, ldl, s));
+        gc.addend = L; gc.ldadd = ldl;
       }
-      gc.lora_T = t_pre; gc.ld_t = ld_t; gc.lora_B = loraB; gc.lora_sec_cols = sec_cols;
-    } else {
-      RF_TRY(unfused_term(gc));
     }
     return rf::gemm_launch(epi, N, K, ngr, gr, s);
   };
@@ -563,28 +608,18 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     g[1].rope_cos = h->rope_cos; g[1].rope_sin = h->rope_sin;
     g[1].norm_q = b.norm_added_q; g[1].norm_k = b.norm_added_k;
     ng = 2;
-    bool cond_lora = false;
     if (use_cond) {
       g[2] = g[0];
       g[2].A = rowp(XN, D, S_cond.row0); g[2].M = S_cond.rows;
       g[2].out = rowp(QKV, D3, S_cond.row0);
       g[2].rope_cos = h->crope_cos; g[2].rope_sin = h->crope_sin;
-      if (h->use_merged) {
-        g[2].W = b.qkv_m;
-      } else if (b.l_q.set || b.l_k.set || b.l_v.set) {
-        cond_lora = true;
-      }
       ng = 3;
     }
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_QKV, D3, D, ng, g, b.qkvA, 3 * kLoraPad, b.qkvB, D, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term_qkv(h, b.qkvA, b.l_q, b.l_k, b.l_v, gc.A, D, S_cond.rows, h->LL, D3, s));
-        gc.addend = h->LL; gc.ldadd = D3;
-        return 0;
-      }));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
-    }
+    merged_w(g, 0, 2, b.qkv_m);
+    const LoraT* dqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
+    LoraGroups lg = lora_groups(b.l_q.set || b.l_k.set || b.l_v.set, 0, S_img.rows, 2);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, dqkv, 3, b.qkvA, b.qkvB, D3));
+    else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // joint attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
     RF_TRY(rf::attention_launch(at, s));
@@ -597,27 +632,17 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     g[1].bias = b.to_add_out.b; g[1].out = rowp(X, D, 0); g[1].ldo = D;
     g[1].res = g[1].out; g[1].ldr = D; g[1].gate = mt + GATE_MSA * D;
     ng = 2;
-    cond_lora = false;
     if (use_cond) {
       g[2] = g[0];
       g[2].A = rowp(ACT, D5, S_cond.row0); g[2].M = S_cond.rows;
       g[2].out = rowp(X, D, S_cond.row0); g[2].res = g[2].out; g[2].gate = mc + GATE_MSA * D;
-      if (h->use_merged) {
-        g[2].W = b.to_out_m;
-      } else if (b.l_out.set) {
-        cond_lora = true;
-      }
       ng = 3;
     }
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_GATE_RES, D, D, ng, g, b.l_out.A, kLoraPad, b.l_out.B, 0, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term(h, b.l_out, gc.A, D5, S_cond.rows, h->LL, D, s));
-        gc.addend = h->LL; gc.ldadd = D;
-        return 0;
-      }));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D, ng, g, s));
-    }
+    merged_w(g, 0, 2, b.to_out_m);
+    const LoraT* dout = &b.l_out;
+    lg = lora_groups(b.l_out.set, 0, S_img.rows, 2);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D, ng, g, lg, &dout, 1, b.l_out.A, b.l_out.B, D));
+    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D, ng, g, s));
     // norm2 + modulate
     RF_TRY(ln3(mt + SCALE_MLP * D, mt + SHIFT_MLP * D, mi + SCALE_MLP * D, mi + SHIFT_MLP * D,
                mc + SCALE_MLP * D, mc + SHIFT_MLP * D));
@@ -645,27 +670,17 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     g[1].A = rowp(ACT, D5, 0) + D; g[1].M = S_txt.rows; g[1].W = b.ffc2.w; g[1].bias = b.ffc2.b;
     g[1].out = rowp(X, D, 0); g[1].res = g[1].out; g[1].gate = mt + GATE_MLP * D;
     ng = 2;
-    cond_lora = false;
     if (use_cond) {
       g[2] = g[0];
       g[2].A = rowp(ACT, D5, S_cond.row0) + D; g[2].M = S_cond.rows;
       g[2].out = rowp(X, D, S_cond.row0); g[2].res = g[2].out; g[2].gate = mc + GATE_MLP * D;
-      if (h->use_merged) {
-        g[2].W = b.ff2_m;
-      } else if (b.l_ff2.set) {
-        cond_lora = true;
-      }
       ng = 3;
     }
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_GATE_RES, D, D4, ng, g, b.l_ff2.A, kLoraPad, b.l_ff2.B, 0, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term(h, b.l_ff2, gc.A, D5, S_cond.rows, h->LL, D, s));
-        gc.addend = h->LL; gc.ldadd = D;
-        return 0;
-      }));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D4, ng, g, s));
-    }
+    merged_w(g, 0, 2, b.ff2_m);
+    const LoraT* dff2 = &b.l_ff2;
+    lg = lora_groups(b.l_ff2.set, 0, S_img.rows, 2);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D4, ng, g, lg, &dff2, 1, b.l_ff2.A, b.l_ff2.B, D));
+    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D4, ng, g, s));
   }
 
   // ================= single-stream blocks (block.py:275-333) =================
@@ -682,59 +697,46 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     g[0].out = QKV; g[0].ldo = D3; g[0].rope_cos = h->rope_cos; g[0].rope_sin = h->rope_sin;
     g[0].norm_q = b.norm_q; g[0].norm_k = b.norm_k;
     ng = 1;
-    bool cond_lora = false;
     if (use_cond) {
       g[1] = g[0];
       g[1].A = rowp(XN, D, S_cond.row0); g[1].M = S_cond.rows;
       g[1].out = rowp(QKV, D3, S_cond.row0);
       g[1].rope_cos = h->crope_cos; g[1].rope_sin = h->crope_sin;
-      if (h->use_merged) {
-        g[1].W = b.qkv_m;
-      } else if (b.l_q.set || b.l_k.set || b.l_v.set) {
-        cond_lora = true;
-      }
       ng = 2;
     }
-    // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp in one launch (both GEMMs read the same XN rows)
-    const bool t4 = use_cond && !h->use_merged && (b.l_q.set || b.l_k.set || b.l_v.set) && b.l_mlp.set &&
-                    rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[ng - 1]);
-    if (t4)
-      RF_TRY(rf::lora_down_launch(g[ng - 1].A, D, S_cond.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad, s));
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_QKV, D3, D, ng, g, b.qkvA, 3 * kLoraPad, b.qkvB, D, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term_qkv(h, b.qkvA, b.l_q, b.l_k, b.l_v, gc.A, D, S_cond.rows, h->LL, D3, s));
-        gc.addend = h->LL; gc.ldadd = D3;
-        return 0;
-      }, t4 ? h->LT : nullptr, 4 * kLoraPad));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
+    merged_w(g, 0, 1, b.qkv_m);
+    const LoraT* sqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
+    LoraGroups lg = lora_groups(b.l_q.set || b.l_k.set || b.l_v.set, 0, S_main.rows, 1);
+    // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp of all LoRA'd rows in one launch (both GEMMs read the
+    // same XN rows; the q|k|v and the MLP-in launches have the same groups)
+    bool t4 = lg.n > 0 && b.l_mlp.set;
+    if (t4) {
+      bool any_fused = false;
+      for (int j = 0; j < lg.n; ++j) any_fused |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[lg.idx[j]]);
+      t4 = any_fused;
     }
+    if (t4)
+      RF_TRY(rf::lora_down_launch(g[lg.idx[0]].A, D, lg.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad, s));
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, sqkv, 3, b.qkvA, b.qkvB, D3, t4 ? h->LT : nullptr,
+                               4 * kLoraPad));
+    else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // proj_mlp + GELU -> ACT[:, D:5D]
     memset(g, 0, sizeof(g));
     g[0].A = XN; g[0].lda = D; g[0].M = S_main.rows; g[0].W = b.mlp.w; g[0].bias = b.mlp.b;
     g[0].out = ACT + D; g[0].ldo = D5;
     ng = 1;
-    cond_lora = false;
     if (use_cond) {
       g[1] = g[0];
       g[1].A = rowp(XN, D, S_cond.row0); g[1].M = S_cond.rows;
       g[1].out = rowp(ACT, D5, S_cond.row0) + D;
-      if (h->use_merged) {
-        g[1].W = b.mlp_m;
-      } else if (b.l_mlp.set) {
-        cond_lora = true;
-      }
       ng = 2;
     }
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_GELU, D4, D, ng, g, b.l_mlp.A, kLoraPad, b.l_mlp.B, 0, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term(h, b.l_mlp, gc.A, D, S_cond.rows, h->LL, D4, s));
-        gc.addend = h->LL; gc.ldadd = D4;
-        return 0;
-      }, t4 ? h->LT + 3 * kLoraPad : nullptr, 4 * kLoraPad));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
-    }
+    merged_w(g, 0, 1, b.mlp_m);
+    const LoraT* smlp = &b.l_mlp;
+    lg = lora_groups(b.l_mlp.set, 0, S_main.rows, 1);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, &smlp, 1, b.l_mlp.A, b.l_mlp.B, D4,
+                               t4 ? h->LT + 3 * kLoraPad : nullptr, 4 * kLoraPad));
+    else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
     // attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
     RF_TRY(rf::attention_launch(at, s));
@@ -743,27 +745,17 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     g[0].A = ACT; g[0].lda = D5; g[0].M = S_main.rows; g[0].W = b.out.w; g[0].bias = b.out.b;
     g[0].out = X; g[0].ldo = D; g[0].res = X; g[0].ldr = D; g[0].gate = mm + 2 * D;
     ng = 1;
-    cond_lora = false;
     if (use_cond) {
       g[1] = g[0];
       g[1].A = rowp(ACT, D5, S_cond.row0); g[1].M = S_cond.rows;
       g[1].out = rowp(X, D, S_cond.row0); g[1].res = g[1].out; g[1].gate = mc + 2 * D;
-      if (h->use_merged) {
-        g[1].W = b.out_m;
-      } else if (b.l_out.set) {
-        cond_lora = true;
-      }
       ng = 2;
     }
-    if (cond_lora) {
-      RF_TRY(gemm_cond_lora(rf::EPI_GATE_RES, D, D5, ng, g, b.l_out.A, kLoraPad, b.l_out.B, 0, [&](rf::GemmGroupArgs& gc) {
-        RF_TRY(lora_term(h, b.l_out, gc.A, D5, S_cond.rows, h->LL, D, s));
-        gc.addend = h->LL; gc.ldadd = D;
-        return 0;
-      }));
-    } else {
-      RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D5, ng, g, s));
-    }
+    merged_w(g, 0, 1, b.out_m);
+    const LoraT* sout = &b.l_out;
+    lg = lora_groups(b.l_out.set, 0, S_main.rows, 1);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D5, ng, g, lg, &sout, 1, b.l_out.A, b.l_out.B, D));
+    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D5, ng, g, s));
   }
 
   // ================= norm_out + proj_out (transformer.py:241-244) =================
@@ -774,6 +766,11 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   g[0].bias = h->proj_out.b; g[0].out = out; g[0].ldo = h->cfg.in_channels;
   RF_TRY(rf::gemm_launch(rf::EPI_BIAS, h->cfg.in_channels, D, 1, g, s));
   return 0;
+}
+
+// fuse_lora mode applies when some group carries a LoRA: the condition stream, or the image under latent_lora
+bool wants_merged(const rf_dit* h, int n_cond) {
+  return (h->flags & 8) != 0 && h->any_lora && (n_cond > 0 || (h->flags & 1) != 0);
 }
 
 void drop_graph(rf_dit* h) {
@@ -787,6 +784,7 @@ void free_geometry(rf_dit* h) {
   for (void* p : h->geo_allocs) cudaFree(p);
   h->geo_allocs.clear();
   h->prepared = false;
+  h->lora_rows = 0;
   h->s_cap_steps = 0;
   h->s_tsteps = nullptr;
   h->s_sigmas = nullptr;
@@ -801,6 +799,20 @@ __global__ void add2_kernel(const bf16* a, const bf16* b, bf16* out, int n) {
 }
 int add2_launch(const bf16* a, const bf16* b, bf16* out, int n, cudaStream_t stream) {
   add2_kernel<<<(n + 255) / 256, 256, 0, stream>>>(a, b, out, n);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+__global__ void add_rows_kernel(bf16* dst, int64_t ldd, const bf16* src, int lds, int cols) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  const int r = blockIdx.y;
+  if (c >= cols) return;
+  bf16* d = dst + r * ldd + c;
+  *d = __float2bfloat16_rn(__bfloat162float(*d) + __bfloat162float(src[static_cast<int64_t>(r) * lds + c]));
+}
+int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, cudaStream_t stream) {
+  if (rows <= 0 || cols <= 0) return 0;
+  add_rows_kernel<<<dim3((cols + 255) / 256, rows), 256, 0, stream>>>(dst, ldd, src, lds, cols);
   RF_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
@@ -1011,10 +1023,6 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     rf::set_error("rf_dit_prepare: bad geometry");
     return -1;
   }
-  if (flags & 1) {
-    rf::set_error("rf_dit_prepare: latent_lora=true (LoRA on image tokens) is not implemented");
-    return -1;
-  }
   if (flags & 2) {
     rf::set_error("rf_dit_prepare: add_cond_attn=true is not implemented");
     return -1;
@@ -1032,11 +1040,14 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (flags & 4) mode = 2;  // union_cond_attn == False wins only if no c_factor...
     if ((flags & 4) && condition_scale != 1.0f) mode = 1;  // c_factor mask overrides (block.py:115)
   }
+  // rows that can carry a LoRA term (LT / LL): the condition stream, plus txt + img under latent_lora (the single
+  // blocks LoRA every main row; the double blocks only the image rows)
+  const int lora_rows = std::max((flags & 1) ? N : n_cond, 1);
   const bool same = h->prepared && h->batch == batch && h->n_txt == n_txt && h->n_img == n_img &&
-                    h->n_cond == n_cond;
+                    h->n_cond == n_cond && h->lora_rows >= lora_rows;
   if (same) drop_graph(h); else free_geometry(h);
   h->flags = flags;
-  h->use_merged = (flags & 8) != 0 && h->any_lora && n_cond > 0;
+  h->use_merged = wants_merged(h, n_cond);
   if (h->use_merged && !h->lora_merged) {
     int mrc = merge_all(h, s);
     if (mrc) return mrc;
@@ -1063,7 +1074,8 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (!(p = A(static_cast<size_t>(N) * 5 * D * 2))) return -2; h->ACT = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MOD = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MODC = static_cast<bf16*>(p);
-    const size_t lrows = static_cast<size_t>(std::max(n_cond, 1));
+    h->lora_rows = lora_rows;
+    const size_t lrows = static_cast<size_t>(lora_rows);
     if (!(p = A(std::max(lrows * 4 * kLoraPad * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LT = static_cast<bf16*>(p);
     if (!(p = A(std::max(lrows * 4 * D * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LL = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(512 + 4 * D) * 2))) return -2; h->emb_tmp = static_cast<bf16*>(p);
@@ -1120,7 +1132,7 @@ static int check_ready(rf_dit* h, const char* who, cudaStream_t s) {
   }
   if (rf_dit_missing_weights(h) != 0) return -4;
   // fuse_lora mode: weights or adapters changed since the last merge -> re-merge before use
-  h->use_merged = (h->flags & 8) != 0 && h->any_lora && h->n_cond > 0;
+  h->use_merged = wants_merged(h, h->n_cond);
   if (h->use_merged && !h->lora_merged) {
     drop_graph(h);
     RF_TRY(merge_all(h, s));
@@ -1190,7 +1202,9 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     h->s_sigmas = static_cast<float*>(p);
     if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
     h->s_mod_all = static_cast<bf16*>(p);
-    if (dev_alloc(h, &p, (static_cast<size_t>(n_steps) * (256 + 3 * h->D) + 256 + 3 * h->D) * 2, true)) return -2;
+    if (dev_alloc(h, &p, (static_cast<size_t>(n_steps) * (256 + 3 * h->D + kLoraPad + 6 * h->D) + 256 + 3 * h->D) * 2,
+                  true))
+      return -2;
     h->s_temb_ws = static_cast<bf16*>(p);
     h->s_cap_steps = n_steps;
     drop_graph(h);  // graph referenced the old arrays

@@ -157,5 +157,7 @@ int euler_step_launch(bf16* x, const bf16* v, const float* sigmas, const int* st
                       cudaStream_t stream);
 int copy_rows_launch(const bf16* src, int lds, bf16* dst, int ldd, int rows, int cols,
                      cudaStream_t stream);
+// dst[r * ldd + c] = bf16(dst[r * ldd + c] + src[r * lds + c]) for r < rows, c < cols
+int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, cudaStream_t stream);
 
 }  // namespace rf

@@ -1,6 +1,9 @@
 #!/usr/bin/env python
-"""Step time of entry B (condition stream + LoRA on condition tokens): the headline tree's step."""
-import os, sys, json, time
+"""Step time of entry B (condition stream + LoRA on condition tokens): the headline tree's step.
+
+Env: LAYERS=double,single (default 19,38), LORA=0|1, LORA_MODE=exact|merged, LATENT_LORA=1 (the LoRA also acts on the
+image and text tokens, model_config["latent_lora"]), STEPS.  Prints the card name and power limit with the timing."""
+import os, sys, json, subprocess, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from reflectionflow_b200 import _lib as L
@@ -12,6 +15,8 @@ dev = torch.device("cuda:0")
 layers = os.environ.get("LAYERS", "19,38").split(",")
 cfg = FluxDiTConfig(num_layers=int(layers[0]), num_single_layers=int(layers[1]))
 use_lora = os.environ.get("LORA", "1") == "1"
+latent_lora = os.environ.get("LATENT_LORA", "0") == "1"
+model_config = {"union_cond_attn": True, "latent_lora": latent_lora}
 pipe = B200FluxPipeline.from_synthetic(cfg, seed=0, device=dev, lora_rank=32 if use_lora else 0)
 if use_lora:
     pipe.transformer.load_lora(synthetic_lora(cfg), mode=os.environ.get("LORA_MODE", "exact"))
@@ -22,7 +27,7 @@ pool = torch.randn(1, 768, generator=g).to(torch.bfloat16)
 cond = Condition("cot", latents=torch.randn(1, 1024, 64, generator=g).to(torch.bfloat16), position_delta=[0, -32])
 K = int(os.environ.get("STEPS", "8"))
 def run(n):
-    return generate(pipe, conditions=[cond], model_config={"union_cond_attn": True}, default_lora=True,
+    return generate(pipe, conditions=[cond], model_config=model_config, default_lora=True,
                     prompt_embeds=txt, pooled_prompt_embeds=pool, latents=lat, height=1024, width=1024,
                     num_inference_steps=n, output_type="latent").images
 run(3); torch.cuda.synchronize()
@@ -30,8 +35,15 @@ e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=Tr
 e0.record(); out = run(K); e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / K
 tf = (57 * 24 * 3072 * 3072 * 5632 + 57 * 4 * 5632 * 5632 * 3072) / 1e12
-print(json.dumps({"entry": "B", "lora": use_lora, "lora_mode": pipe.transformer.lora_mode, "n_tok": 5632, "ms_per_step": ms, "steps_per_s": 1e3 / ms,
-                  "step_tflop": tf, "tflops": tf / ms * 1e3, "finite": bool(torch.isfinite(out.float()).all())}))
+try:
+    power_limit = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
+                                 capture_output=True, text=True, timeout=30).stdout.strip()
+except Exception:
+    power_limit = "unknown"
+print(json.dumps({"entry": "B", "lora": use_lora, "lora_mode": pipe.transformer.lora_mode, "latent_lora": latent_lora,
+                  "n_tok": 5632, "ms_per_step": ms, "steps_per_s": 1e3 / ms, "step_tflop": tf, "tflops": tf / ms * 1e3,
+                  "finite": bool(torch.isfinite(out.float()).all()), "gpu": torch.cuda.get_device_name(dev),
+                  "power_limit": power_limit}))
 from reflectionflow_b200.transformer import tranformer_forward
 m = pipe.transformer
 ids_i = pipe._prepare_latent_image_ids(1, 64, 64, dev, torch.bfloat16)
@@ -40,11 +52,12 @@ ctok, cids, _ = cond.encode(pipe)
 kw = dict(hidden_states=lat, encoder_hidden_states=txt, pooled_projections=pool,
           timestep=torch.tensor([0.5], dtype=torch.bfloat16), img_ids=ids_i, txt_ids=ids_t,
           guidance=torch.tensor([3.5]), return_dict=False)
-tranformer_forward(m, ctok, cids, None, {}, 0, **kw)
+tranformer_forward(m, ctok, cids, None, model_config, 0, **kw)
 torch.cuda.synchronize()
 L.profile_start()
-tranformer_forward(m, ctok, cids, None, {}, 0, **kw)
+tranformer_forward(m, ctok, cids, None, model_config, 0, **kw)
 prof = L.profile_stop()
 tot = sum(v["ms"] for v in prof.values())
+print(f"  one eager forward: {sum(v['launches'] for v in prof.values())} launches, {tot:.3f} ms of kernel time")
 for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"]):
     print(f"  {k:20s} launches {v['launches']:4d}  ms {v['ms']:7.3f}  share {v['ms']/tot:.3f}")
