@@ -123,7 +123,9 @@ typedef struct rf_dit_config {
   int joint_attention_dim; /* 4096 (T5 width)                       */
   int pooled_projection_dim; /* 768 (CLIP pooled width)             */
   int guidance_embeds;     /* 1 for FLUX.1-dev                      */
-  int lora_rank;           /* 0 = no LoRA storage; else max rank (<= 64) of the LoRA (cond tokens, + latent_lora) */
+  int lora_rank;           /* 0 = no LoRA storage; else max rank (<= 128) of the LoRA (cond tokens, + latent_lora).
+                              Ranks <= 64 are stored zero-padded to 64, ranks 65..128 to 128 (one resp. two 64-deep
+                              low-rank k-blocks per fused GEMM tile) */
 } rf_dit_config;
 
 int rf_dit_create(const rf_dit_config* cfg, rf_dit** out);
@@ -139,12 +141,23 @@ int rf_dit_load_weight(rf_dit* h, const char* key, const void* src, int64_t nume
  * target list train_flux/config.yaml:53).  module = diffusers module path without ".weight"
  * (e.g. "single_transformer_blocks.0.proj_out"); A: [r, in_features] bf16, B: [out_features, r]
  * bf16 (device); in_/out_features are checked against the target Linear (a mismatched adapter
- * file is an error, not an out-of-bounds read); scale = lora_alpha / r.  Applied to condition
- * tokens only unless latent_lora is set in rf_dit_prepare (lora_controller.py:5-42); with it, to every
- * token that passes the target: the image stream of the double blocks, the txt + img rows of the single
- * blocks, and the image / main-row adaLN modulation (norm1.linear / norm.linear of temb). */
+ * file is an error, not an out-of-bounds read); r <= lora_rank; scale = that target's lora_alpha / r,
+ * any finite value (NaN / inf are refused).  Applied to condition tokens only unless latent_lora is set in
+ * rf_dit_prepare (lora_controller.py:5-42); with it, to every token that passes the target: the image stream
+ * of the double blocks, the txt + img rows of the single blocks, and the image / main-row adaLN modulation
+ * (norm1.linear / norm.linear of temb).
+ * Arithmetic (peft): y = bf16( bf16(x W^T + b) + bf16( bf16(T B^T) * s ) ), T = bf16(x A^T), with s the
+ * target's effective scaling float(scale * call_scale) (product in double, as peft's `scaling *= scale`;
+ * call_scale from rf_dit_set_lora_scale).  A target whose s is 0 adds nothing and runs no launch. */
 int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B, int r,
                     int in_features, int out_features, float scale);
+
+/* The call-level LoRA multiplier (diffusers' joint_attention_kwargs["scale"], scale_lora_layers): every
+ * target's scaling is multiplied by `scale` from the next rf_dit_forward / rf_dit_denoise on; 1 by default,
+ * any finite value.  It stays until changed.  A denoise call whose scale differs from the one its captured
+ * step was built with re-captures the step (one capture + instantiate); in merged mode (rf_dit_prepare flag
+ * bit3) the merged weights are re-merged at the new scale (one pass over the LoRA target weights). */
+int rf_dit_set_lora_scale(rf_dit* h, double scale);
 
 /* Number of parameters still missing (0 = ready); names via rf_last_error(). */
 int rf_dit_missing_weights(rf_dit* h);

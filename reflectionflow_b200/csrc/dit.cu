@@ -28,7 +28,7 @@
 #include "rf_internal.h"
 
 namespace rf {
-int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R,
+int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R, float scale,
                       cudaStream_t stream);
 int add2_launch(const bf16* a, const bf16* b, bf16* out, int n, cudaStream_t stream);
 int select_row_launch(const bf16* table, int64_t row_elems, const int* row, bf16* out,
@@ -54,11 +54,12 @@ struct Lin {  // views into the weight arena
   bf16* b = nullptr;
 };
 
-struct LoraT {  // zero-padded rank-64 factors of one target
-  bf16* A = nullptr;  // [64, in]
-  bf16* B = nullptr;  // [out, 64]
+struct LoraT {  // factors of one target, rank zero-padded to the handle's lora_pad
+  bf16* A = nullptr;  // [lora_pad, in]
+  bf16* B = nullptr;  // [out, lora_pad]
   int in = 0, out = 0;
   bool set = false;
+  double scale = 1.0;  // lora_alpha / r
 };
 // (merged weights W + B A of a whole packed projection live in the block structs: *_m)
 
@@ -66,8 +67,8 @@ struct DoubleBlk {
   Lin qkv, add_qkv, to_out, to_add_out, ff1, ff2, ffc1, ffc2;
   bf16 *norm_q, *norm_k, *norm_added_q, *norm_added_k;
   LoraT l_norm1, l_q, l_k, l_v, l_out, l_ff2;
-  bf16* qkvA = nullptr;  // [192, D] = stacked A of to_q/to_k/to_v
-  bf16* qkvB = nullptr;  // [3D, 64] = stacked B (rows of the packed q|k|v projection)
+  bf16* qkvA = nullptr;  // [3 lora_pad, D] = stacked A of to_q/to_k/to_v
+  bf16* qkvB = nullptr;  // [3D, lora_pad] = stacked B (rows of the packed q|k|v projection)
   bf16 *qkv_m = nullptr, *to_out_m = nullptr, *ff2_m = nullptr;  // merged W + B A (fuse_lora mode)
 };
 struct SingleBlk {
@@ -78,8 +79,6 @@ struct SingleBlk {
   bf16* qkvB = nullptr;
   bf16 *qkv_m = nullptr, *mlp_m = nullptr, *out_m = nullptr;
 };
-
-constexpr int kLoraPad = 64;
 
 }  // namespace
 
@@ -100,7 +99,13 @@ struct rf_dit {
   std::vector<DoubleBlk> dbl;
   std::vector<SingleBlk> sgl;
   bool any_lora = false;
-  bool lora_merged = false;   // merged copies are current
+  // LoRA rank padding: 64 for lora_rank <= 64, else 128 (one or two 64-deep low-rank k-blocks per fused tile)
+  int lora_pad = 64;
+  // rf_dit_set_lora_scale: peft's call-level multiplier (joint_attention_kwargs["scale"]); a target's effective
+  // scaling is float(scale * call_scale), formed in double like peft's `scaling *= scale`
+  double call_scale = 1.0;
+  bool lora_merged = false;   // merged copies are current for merged_call_scale
+  double merged_call_scale = 1.0;
   bool use_merged = false;    // rf_dit_prepare flag bit 3
   bf16* x_emb_m = nullptr;
   // ---- geometry
@@ -129,9 +134,15 @@ struct rf_dit {
   cudaStream_t own_stream = nullptr;  // capture is illegal on the legacy default stream
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   int64_t graph_kernels = 0;  // kernel launches inside one captured step
+  double graph_call_scale = 1.0;  // call_scale the captured step was built with (kernel parameters, launch list)
 };
 
 namespace {
+
+// the fp32 scaling peft multiplies the bf16 low-rank term of target t by
+float lora_eff(const rf_dit* h, const LoraT& t) { return static_cast<float>(t.scale * h->call_scale); }
+// a target whose effective scaling is 0 adds exactly nothing: it runs no launch at all
+bool lora_on(const rf_dit* h, const LoraT& t) { return t.set && lora_eff(h, t) != 0.f; }
 
 int dev_alloc(rf_dit* h, void** p, size_t bytes, bool geometry = false) {
   RF_CHECK_CUDA(cudaMalloc(p, bytes ? bytes : 16));
@@ -172,17 +183,18 @@ void new_lora(rf_dit* h, Arena& ar, const std::string& mod, LoraT& t, int out, i
   if (h->cfg.lora_rank <= 0) return;
   t.in = in;
   t.out = out;
-  t.A = A_view ? A_view : ar.take(static_cast<int64_t>(kLoraPad) * in);
-  t.B = B_view ? B_view : ar.take(static_cast<int64_t>(out) * kLoraPad);
+  const int pad = h->lora_pad;
+  t.A = A_view ? A_view : ar.take(static_cast<int64_t>(pad) * in);
+  t.B = B_view ? B_view : ar.take(static_cast<int64_t>(out) * pad);
   // unset targets must contribute exactly zero (a q-only adapter still runs the stacked q|k|v path)
-  if (t.A) cudaMemset(t.A, 0, static_cast<size_t>(kLoraPad) * in * 2);
-  if (t.B) cudaMemset(t.B, 0, static_cast<size_t>(out) * kLoraPad * 2);
+  if (t.A) cudaMemset(t.A, 0, static_cast<size_t>(pad) * in * 2);
+  if (t.B) cudaMemset(t.B, 0, static_cast<size_t>(out) * pad * 2);
   h->lora_slots[mod] = &t;
 }
 
 int build_storage(rf_dit* h) {
   const rf_dit_config& c = h->cfg;
-  const int D = h->D;
+  const int D = h->D, lpad = h->lora_pad;
   Arena ar{h};
   h->x_emb = new_lin(h, ar, "x_embedder", D, c.in_channels);
   new_lora(h, ar, "x_embedder", h->l_x_emb, D, c.in_channels);
@@ -215,8 +227,8 @@ int build_storage(rf_dit* h) {
     const char* nm[3] = {"to_q", "to_k", "to_v"};
     const char* an[3] = {"add_q_proj", "add_k_proj", "add_v_proj"};
     if (c.lora_rank > 0) {
-      b.qkvA = ar.take(static_cast<int64_t>(3 * kLoraPad) * D);
-      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * kLoraPad);
+      b.qkvA = ar.take(static_cast<int64_t>(3 * lpad) * D);
+      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * lpad);
     }
     LoraT* lq[3] = {&b.l_q, &b.l_k, &b.l_v};
     for (int j = 0; j < 3; ++j) {
@@ -224,8 +236,8 @@ int build_storage(rf_dit* h) {
       reg_lin(h, p + "attn." + an[j], b.add_qkv.w + static_cast<int64_t>(j) * D * D,
               b.add_qkv.b + j * D, D, D);
       new_lora(h, ar, p + "attn." + nm[j], *lq[j], D, D,
-               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * kLoraPad * D : nullptr,
-               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * kLoraPad : nullptr);
+               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * lpad * D : nullptr,
+               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * lpad : nullptr);
     }
     b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
     b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
@@ -252,22 +264,22 @@ int build_storage(rf_dit* h) {
     if (c.lora_rank > 0) {
       // A factors of to_q | to_k | to_v | proj_mlp stacked: all four read the same normalised tokens, so
       // ONE down-projection launch (NT = 256) serves the q|k|v and the MLP-in GEMMs of the block
-      b.qkvA = ar.take(static_cast<int64_t>(4 * kLoraPad) * D);
-      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * kLoraPad);
+      b.qkvA = ar.take(static_cast<int64_t>(4 * lpad) * D);
+      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * lpad);
     }
     const char* nm[3] = {"to_q", "to_k", "to_v"};
     LoraT* lq[3] = {&b.l_q, &b.l_k, &b.l_v};
     for (int j = 0; j < 3; ++j) {
       reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
       new_lora(h, ar, p + "attn." + nm[j], *lq[j], D, D,
-               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * kLoraPad * D : nullptr,
-               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * kLoraPad : nullptr);
+               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * lpad * D : nullptr,
+               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * lpad : nullptr);
     }
     b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
     b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
     b.mlp = new_lin(h, ar, p + "proj_mlp", 4 * D, D);
     new_lora(h, ar, p + "proj_mlp", b.l_mlp, 4 * D, D,
-             b.qkvA ? b.qkvA + static_cast<int64_t>(3 * kLoraPad) * D : nullptr);
+             b.qkvA ? b.qkvA + static_cast<int64_t>(3 * lpad) * D : nullptr);
     b.out = new_lin(h, ar, p + "proj_out", D, 5 * D);
     new_lora(h, ar, p + "proj_out", b.l_out, D, 5 * D);
   }
@@ -330,34 +342,39 @@ int compute_temb(rf_dit* h, const bf16* t, const int* step, const bf16* guid, co
 // runs.  Otherwise T is computed here into LT.
 int lora_term(rf_dit* h, const LoraT* const* ls, int n, const bf16* A_all, const bf16* x, int ldx, int rows,
               const bf16* T, int ld_t, bf16* L, int ldl, cudaStream_t s) {
+  const int lpad = h->lora_pad;
   rf::GemmGroupArgs g[3];
   if (T == nullptr) {
     memset(g, 0, sizeof(g));
-    g[0].A = x; g[0].lda = ldx; g[0].M = rows; g[0].W = A_all; g[0].out = h->LT; g[0].ldo = n * kLoraPad;
-    RF_TRY(rf::gemm_launch(rf::EPI_BIAS, n * kLoraPad, ls[0]->in, 1, g, s));
+    g[0].A = x; g[0].lda = ldx; g[0].M = rows; g[0].W = A_all; g[0].out = h->LT; g[0].ldo = n * lpad;
+    RF_TRY(rf::gemm_launch(rf::EPI_BIAS, n * lpad, ls[0]->in, 1, g, s));
     T = h->LT;
-    ld_t = n * kLoraPad;
+    ld_t = n * lpad;
   }
   memset(g, 0, sizeof(g));
+  bool scaled = false;  // peft's bf16(bf16(T B^T) * scaling): the scale is the up-projection's output scale
   for (int j = 0; j < n; ++j) {
-    g[j].A = T + j * kLoraPad; g[j].lda = ld_t; g[j].M = rows;
+    g[j].A = T + j * lpad; g[j].lda = ld_t; g[j].M = rows;
     g[j].W = ls[j]->B; g[j].out = L + static_cast<int64_t>(j) * ls[j]->out; g[j].ldo = ldl;
+    g[j].lora_scale[0] = lora_eff(h, *ls[j]);
+    scaled |= g[j].lora_scale[0] != 1.f;
   }
-  return rf::gemm_launch(rf::EPI_BIAS, ls[0]->out, kLoraPad, n, g, s);
+  return rf::gemm_launch(scaled ? rf::EPI_SCALE : rf::EPI_BIAS, ls[0]->out, lpad, n, g, s);
 }
 
 // The low-rank term of the adaLN Linears (norm1.linear of the double blocks, norm.linear of the single blocks)
 // added to their sections of `batch` modulation rows: mod[b * ld_mod + section] += bf16(bf16(silu(emb_b) A^T) B^T)
 // (peft: bf16(y + L)).  M = batch is tiny: two batched GEMVs and one strided add per target.
-// tvec: [batch, 64], lvec: [batch, 6D] scratch.
+// The scaling is applied in the add: mod += bf16(L * scaling).
+// tvec: [batch, lora_pad], lvec: [batch, 6D] scratch.
 int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bf16* mod, int64_t ld_mod, bf16* tvec, bf16* lvec,
                  cudaStream_t s) {
-  const int D = h->D;
+  const int D = h->D, lpad = h->lora_pad;
   auto one = [&](const LoraT& t, int64_t off) -> int {
-    if (!t.set) return 0;
-    RF_TRY(rf::gemv_launch(emb, D, batch, t.A, nullptr, tvec, kLoraPad, kLoraPad, D, 1, s));
-    RF_TRY(rf::gemv_launch(tvec, kLoraPad, batch, t.B, nullptr, lvec, t.out, t.out, kLoraPad, 0, s));
-    return rf::add_rows_launch(mod + off, ld_mod, lvec, t.out, batch, t.out, s);
+    if (!lora_on(h, t)) return 0;
+    RF_TRY(rf::gemv_launch(emb, D, batch, t.A, nullptr, tvec, lpad, lpad, D, 1, s));
+    RF_TRY(rf::gemv_launch(tvec, lpad, batch, t.B, nullptr, lvec, t.out, t.out, lpad, 0, s));
+    return rf::add_rows_launch(mod + off, ld_mod, lvec, t.out, batch, t.out, lora_eff(h, t), s);
   };
   for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1, mod_double(h, i, 0, 0)));
   for (int i = 0; i < h->cfg.num_single_layers; ++i) RF_TRY(one(h->sgl[i].l_norm, mod_single(h, i, 0)));
@@ -372,7 +389,7 @@ int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
   RF_TRY(rf::gemv_launch(h->ctemb, D, 1, h->modW, h->modB, h->MODC, static_cast<int>(h->n_mod),
                          static_cast<int>(h->n_mod), D, 1, s));
   if (!h->any_lora) return 0;
-  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb)
+  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb); tvec [1, lora_pad <= 256] at the front of LT
   return add_mod_lora(h, h->ctemb, 1, h->MODC, h->n_mod, h->LT, h->LT + 256, s);
 }
 
@@ -391,7 +408,7 @@ int merge_one(rf_dit* h, const LoraT& t, const bf16* W, bf16** Wm, int rows_off,
                                   cudaMemcpyDeviceToDevice, s));
     return 0;
   }
-  return rf::lora_merge_launch(W + off, t.A, t.B, *Wm + off, t.out, t.in, kLoraPad, s);
+  return rf::lora_merge_launch(W + off, t.A, t.B, *Wm + off, t.out, t.in, h->lora_pad, lora_eff(h, t), s);
 }
 int merge_all(rf_dit* h, cudaStream_t s) {
   const int D = h->D;
@@ -411,6 +428,7 @@ int merge_all(rf_dit* h, cudaStream_t s) {
     RF_TRY(merge_one(h, b.l_out, b.out.w, &b.out_m, 0, D, s));
   }
   h->lora_merged = true;
+  h->merged_call_scale = h->call_scale;
   return 0;
 }
 
@@ -421,7 +439,7 @@ int merge_all(rf_dit* h, cudaStream_t s) {
 int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16* guid,
                          const bf16* pooled, cudaStream_t s) {
   const int D = h->D;
-  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c | [n,64] | [n,6D] (LoRA)
+  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c | [n,lora_pad] | [n,6D] (LoRA)
   bf16* ws = h->s_temb_ws;
   bf16* tp = ws;
   bf16* tmp = tp + static_cast<int64_t>(n_steps) * 256;
@@ -448,8 +466,8 @@ int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16*
   // latent_lora: the adaLN LoRA of the image stream (double blocks) / of the txt+img rows (single blocks) acts on
   // silu(temb_i), which every step knows before the loop: its term joins the table here too
   if ((h->flags & 1) && h->any_lora) {
-    bf16* tvec = c + D;                                      // [n, 64]
-    bf16* lvec = tvec + static_cast<int64_t>(n_steps) * kLoraPad;  // [n, 6D]
+    bf16* tvec = c + D;                                               // [n, lora_pad]
+    bf16* lvec = tvec + static_cast<int64_t>(n_steps) * h->lora_pad;  // [n, 6D]
     RF_TRY(add_mod_lora(h, temb, n_steps, h->s_mod_all, h->n_mod, tvec, lvec, s));
   }
   return 0;
@@ -463,7 +481,7 @@ struct StreamRows {
 int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16* pooled,
                     const bf16* tstep, const int* step_idx, const bf16* guid, const bf16* cond_lat,
                     bf16* out, cudaStream_t s, const bf16* mod_all = nullptr) {
-  const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D;
+  const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D, lpad = h->lora_pad;
   const bool use_cond = h->n_cond > 0;
   // latent_lora (lora_controller.py:5-9): the LoRA also acts on the image stream of the double blocks and on the
   // txt + img rows of the single blocks (the text stream of the double blocks has no LoRA target)
@@ -486,7 +504,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   if (h->use_merged) {
     if (ll) g[0].W = h->x_emb_m;
     if (use_cond) g[1].W = h->x_emb_m;
-  } else if (h->l_x_emb.set) {
+  } else if (lora_on(h, h->l_x_emb)) {
     // K = 64, EPI_BIAS: the unfused low-rank term, each LoRA'd group's L in its own rows of LL
     const LoraT* xl = &h->l_x_emb;
     int row = 0;
@@ -556,15 +574,17 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     for (int j = 0; j < lg.n; ++j) any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, gr[lg.idx[j]]));
     if (any_fused && t_pre == nullptr) {
       const rf::GemmGroupArgs& g0 = gr[lg.idx[0]];
-      RF_TRY(rf::lora_down_launch(g0.A, g0.lda, lg.rows, K, A_all, nls * kLoraPad, h->LT, nls * kLoraPad, s));
+      RF_TRY(rf::lora_down_launch(g0.A, g0.lda, lg.rows, K, A_all, nls * lpad, h->LT, nls * lpad, s));
       t_pre = h->LT;
-      ld_t = nls * kLoraPad;
+      ld_t = nls * lpad;
     }
     for (int j = 0; j < lg.n; ++j) {
       rf::GemmGroupArgs& gc = gr[lg.idx[j]];
       const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(lg.row[j]) * ld_t : nullptr;
       if (fused[j]) {
         gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = B_all; gc.lora_sec_cols = nls > 1 ? ls[0]->out : 0;
+        gc.lora_pad = lpad;
+        for (int k = 0; k < nls; ++k) gc.lora_scale[k] = lora_eff(h, *ls[k]);
       } else {
         bf16* L = rowp(h->LL, ldl, lg.row[j]);
         RF_TRY(lora_term(h, ls, nls, A_all, gc.A, gc.lda, gc.M, t_rows, ld_t, L, ldl, s));
@@ -617,7 +637,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 2, b.qkv_m);
     const LoraT* dqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraGroups lg = lora_groups(b.l_q.set || b.l_k.set || b.l_v.set, 0, S_img.rows, 2);
+    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_img.rows, 2);
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, dqkv, 3, b.qkvA, b.qkvB, D3));
     else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // joint attention -> ACT[:, 0:D]
@@ -640,7 +660,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 2, b.to_out_m);
     const LoraT* dout = &b.l_out;
-    lg = lora_groups(b.l_out.set, 0, S_img.rows, 2);
+    lg = lora_groups(lora_on(h, b.l_out), 0, S_img.rows, 2);
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D, ng, g, lg, &dout, 1, b.l_out.A, b.l_out.B, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D, ng, g, s));
     // norm2 + modulate
@@ -678,7 +698,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 2, b.ff2_m);
     const LoraT* dff2 = &b.l_ff2;
-    lg = lora_groups(b.l_ff2.set, 0, S_img.rows, 2);
+    lg = lora_groups(lora_on(h, b.l_ff2), 0, S_img.rows, 2);
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D4, ng, g, lg, &dff2, 1, b.l_ff2.A, b.l_ff2.B, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D4, ng, g, s));
   }
@@ -706,19 +726,19 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.qkv_m);
     const LoraT* sqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraGroups lg = lora_groups(b.l_q.set || b.l_k.set || b.l_v.set, 0, S_main.rows, 1);
+    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_main.rows, 1);
     // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp of all LoRA'd rows in one launch (both GEMMs read the
     // same XN rows; the q|k|v and the MLP-in launches have the same groups)
-    bool t4 = lg.n > 0 && b.l_mlp.set;
+    bool t4 = lg.n > 0 && lora_on(h, b.l_mlp);
     if (t4) {
       bool any_fused = false;
       for (int j = 0; j < lg.n; ++j) any_fused |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[lg.idx[j]]);
       t4 = any_fused;
     }
     if (t4)
-      RF_TRY(rf::lora_down_launch(g[lg.idx[0]].A, D, lg.rows, D, b.qkvA, 4 * kLoraPad, h->LT, 4 * kLoraPad, s));
+      RF_TRY(rf::lora_down_launch(g[lg.idx[0]].A, D, lg.rows, D, b.qkvA, 4 * lpad, h->LT, 4 * lpad, s));
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, sqkv, 3, b.qkvA, b.qkvB, D3, t4 ? h->LT : nullptr,
-                               4 * kLoraPad));
+                               4 * lpad));
     else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // proj_mlp + GELU -> ACT[:, D:5D]
     memset(g, 0, sizeof(g));
@@ -733,9 +753,9 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.mlp_m);
     const LoraT* smlp = &b.l_mlp;
-    lg = lora_groups(b.l_mlp.set, 0, S_main.rows, 1);
+    lg = lora_groups(lora_on(h, b.l_mlp), 0, S_main.rows, 1);
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, &smlp, 1, b.l_mlp.A, b.l_mlp.B, D4,
-                               t4 ? h->LT + 3 * kLoraPad : nullptr, 4 * kLoraPad));
+                               t4 ? h->LT + 3 * lpad : nullptr, 4 * lpad));
     else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
     // attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
@@ -753,7 +773,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.out_m);
     const LoraT* sout = &b.l_out;
-    lg = lora_groups(b.l_out.set, 0, S_main.rows, 1);
+    lg = lora_groups(lora_on(h, b.l_out), 0, S_main.rows, 1);
     if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D5, ng, g, lg, &sout, 1, b.l_out.A, b.l_out.B, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D5, ng, g, s));
   }
@@ -772,6 +792,8 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
 bool wants_merged(const rf_dit* h, int n_cond) {
   return (h->flags & 8) != 0 && h->any_lora && (n_cond > 0 || (h->flags & 1) != 0);
 }
+// the merged copies hold W + (B A) * scaling for the current weights, adapters and call scale
+bool merged_current(const rf_dit* h) { return h->lora_merged && h->merged_call_scale == h->call_scale; }
 
 void drop_graph(rf_dit* h) {
   if (h->graph_exec) {
@@ -803,16 +825,18 @@ int add2_launch(const bf16* a, const bf16* b, bf16* out, int n, cudaStream_t str
   count_launch();
   return 0;
 }
-__global__ void add_rows_kernel(bf16* dst, int64_t ldd, const bf16* src, int lds, int cols) {
+__global__ void add_rows_kernel(bf16* dst, int64_t ldd, const bf16* src, int lds, int cols, float scale) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   const int r = blockIdx.y;
   if (c >= cols) return;
   bf16* d = dst + r * ldd + c;
-  *d = __float2bfloat16_rn(__bfloat162float(*d) + __bfloat162float(src[static_cast<int64_t>(r) * lds + c]));
+  const float v = __bfloat162float(__float2bfloat16_rn(__bfloat162float(src[static_cast<int64_t>(r) * lds + c]) * scale));
+  *d = __float2bfloat16_rn(__bfloat162float(*d) + v);
 }
-int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, cudaStream_t stream) {
+int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, float scale,
+                    cudaStream_t stream) {
   if (rows <= 0 || cols <= 0) return 0;
-  add_rows_kernel<<<dim3((cols + 255) / 256, rows), 256, 0, stream>>>(dst, ldd, src, lds, cols);
+  add_rows_kernel<<<dim3((cols + 255) / 256, rows), 256, 0, stream>>>(dst, ldd, src, lds, cols, scale);
   RF_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
@@ -847,10 +871,11 @@ int f32_to_bf16_launch(const float* src, bf16* dst, int n, cudaStream_t stream) 
   count_launch();
   return 0;
 }
-// Wm[n, k] = bf16( W[n, k] + sum_r B[n, r] * A[r, k] ): what peft's fuse_lora / merge() produces
+// Wm[n, k] = bf16( W[n, k] + scale * sum_r B[n, r] * A[r, k] ): what peft's fuse_lora / merge() produces
+// (delta = (B A) * scaling, get_delta_weight), with one rounding
 __global__ void lora_merge_kernel(const bf16* __restrict__ W, const bf16* __restrict__ A,
                                   const bf16* __restrict__ B, bf16* __restrict__ Wm, int N, int K,
-                                  int R) {
+                                  int R, float scale) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = blockIdx.y;
   if (k >= K) return;
@@ -859,12 +884,12 @@ __global__ void lora_merge_kernel(const bf16* __restrict__ W, const bf16* __rest
     acc = fmaf(__bfloat162float(B[static_cast<size_t>(n) * R + r]),
                __bfloat162float(A[static_cast<size_t>(r) * K + k]), acc);
   const size_t i = static_cast<size_t>(n) * K + k;
-  Wm[i] = __float2bfloat16_rn(__bfloat162float(W[i]) + acc);
+  Wm[i] = __float2bfloat16_rn(__bfloat162float(W[i]) + __fmul_rn(scale, acc));
 }
-int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R,
+int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R, float scale,
                       cudaStream_t stream) {
   dim3 grid((K + 255) / 256, N);
-  lora_merge_kernel<<<grid, 256, 0, stream>>>(W, A, B, Wm, N, K, R);
+  lora_merge_kernel<<<grid, 256, 0, stream>>>(W, A, B, Wm, N, K, R, scale);
   RF_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return 0;
@@ -894,18 +919,23 @@ int rf_dit_create(const rf_dit_config* cfg, rf_dit** out) {
     rf::set_error("rf_dit_create: null argument");
     return -1;
   }
+  if (cfg->lora_rank < 0 || cfg->lora_rank > 128) {
+    rf::set_error("rf_dit_create: lora_rank must be 0..128, got " + std::to_string(cfg->lora_rank));
+    return -1;
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     rf::set_error("rf_dit_create: no CUDA device (this library has no CPU fallback)");
     return -3;
   }
   if (cfg->num_heads <= 0 || cfg->in_channels % 64 != 0 || cfg->joint_attention_dim % 64 != 0 ||
-      cfg->pooled_projection_dim % 8 != 0 || cfg->lora_rank < 0 || cfg->lora_rank > kLoraPad) {
+      cfg->pooled_projection_dim % 8 != 0) {
     rf::set_error("rf_dit_create: unsupported config");
     return -1;
   }
   rf_dit* h = new rf_dit();
   h->cfg = *cfg;
+  h->lora_pad = cfg->lora_rank <= 64 ? 64 : 128;
   h->D = cfg->num_heads * 128;
   if (h->D % 256 != 0 || h->D > 3072) {
     rf::set_error("rf_dit_create: inner dim must be a multiple of 256, <= 3072");
@@ -971,14 +1001,16 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
     rf::set_error(std::string("rf_dit_set_lora: not a LoRA target (or lora_rank == 0): ") + module);
     return -4;
   }
-  if (r <= 0 || r > kLoraPad) {
-    rf::set_error("rf_dit_set_lora: rank must be 1..64");
+  if (r <= 0 || r > h->cfg.lora_rank) {
+    rf::set_error("rf_dit_set_lora: rank " + std::to_string(r) + " of " + module + " exceeds the handle's lora_rank " +
+                  std::to_string(h->cfg.lora_rank));
     return -1;
   }
-  if (scale != 1.0f) {
-    rf::set_error("rf_dit_set_lora: only scaling == 1 (lora_alpha == r, train_flux/config.yaml:50-51) is bit-faithful; other scalings unsupported");
+  if (!std::isfinite(scale)) {
+    rf::set_error(std::string("rf_dit_set_lora: scale (lora_alpha / r) of ") + module + " must be finite");
     return -1;
   }
+  const int lpad = h->lora_pad;
   LoraT& t = *it->second;
   if (in_features != t.in || out_features != t.out) {
     rf::set_error(std::string("rf_dit_set_lora: ") + module + " expects A [r, " + std::to_string(t.in) +
@@ -986,15 +1018,31 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
                   " out=" + std::to_string(out_features));
     return -4;
   }
-  RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(kLoraPad) * t.in * 2));
-  RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * kLoraPad * 2));
+  RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(lpad) * t.in * 2));
+  RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * lpad * 2));
   RF_CHECK_CUDA(cudaMemcpy(t.A, A, static_cast<size_t>(r) * t.in * 2, cudaMemcpyDeviceToDevice));
-  RF_CHECK_CUDA(cudaMemcpy2D(t.B, kLoraPad * 2, B, static_cast<size_t>(r) * 2,
+  RF_CHECK_CUDA(cudaMemcpy2D(t.B, lpad * 2, B, static_cast<size_t>(r) * 2,
                              static_cast<size_t>(r) * 2, t.out, cudaMemcpyDeviceToDevice));
   t.set = true;
+  t.scale = scale;
   h->any_lora = true;
   h->lora_merged = false;
   drop_graph(h);  // the captured step may predate this adapter (different launch list)
+  return 0;
+}
+
+int rf_dit_set_lora_scale(rf_dit* h, double scale) {
+  if (!h) {
+    rf::set_error("rf_dit_set_lora_scale: null handle");
+    return -1;
+  }
+  if (!std::isfinite(scale)) {
+    rf::set_error("rf_dit_set_lora_scale: scale must be finite");
+    return -1;
+  }
+  // takes effect at the next call: the merged copies are re-merged (check_ready) and the captured step is
+  // re-captured (rf_dit_denoise) when they were built for another scale
+  h->call_scale = scale;
   return 0;
 }
 
@@ -1048,7 +1096,7 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
   if (same) drop_graph(h); else free_geometry(h);
   h->flags = flags;
   h->use_merged = wants_merged(h, n_cond);
-  if (h->use_merged && !h->lora_merged) {
+  if (h->use_merged && !merged_current(h)) {
     int mrc = merge_all(h, s);
     if (mrc) return mrc;
   }
@@ -1076,7 +1124,7 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MODC = static_cast<bf16*>(p);
     h->lora_rows = lora_rows;
     const size_t lrows = static_cast<size_t>(lora_rows);
-    if (!(p = A(std::max(lrows * 4 * kLoraPad * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LT = static_cast<bf16*>(p);
+    if (!(p = A(std::max(lrows * 4 * h->lora_pad * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LT = static_cast<bf16*>(p);
     if (!(p = A(std::max(lrows * 4 * D * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LL = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(512 + 4 * D) * 2))) return -2; h->emb_tmp = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->temb = static_cast<bf16*>(p);
@@ -1133,7 +1181,7 @@ static int check_ready(rf_dit* h, const char* who, cudaStream_t s) {
   if (rf_dit_missing_weights(h) != 0) return -4;
   // fuse_lora mode: weights or adapters changed since the last merge -> re-merge before use
   h->use_merged = wants_merged(h, h->n_cond);
-  if (h->use_merged && !h->lora_merged) {
+  if (h->use_merged && !merged_current(h)) {
     drop_graph(h);
     RF_TRY(merge_all(h, s));
   }
@@ -1202,7 +1250,7 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     h->s_sigmas = static_cast<float*>(p);
     if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
     h->s_mod_all = static_cast<bf16*>(p);
-    if (dev_alloc(h, &p, (static_cast<size_t>(n_steps) * (256 + 3 * h->D + kLoraPad + 6 * h->D) + 256 + 3 * h->D) * 2,
+    if (dev_alloc(h, &p, (static_cast<size_t>(n_steps) * (256 + 3 * h->D + h->lora_pad + 6 * h->D) + 256 + 3 * h->D) * 2,
                   true))
       return -2;
     h->s_temb_ws = static_cast<bf16*>(p);
@@ -1237,7 +1285,11 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     }
     RF_TRY(precompute_step_mods(h, n_steps, h->s_tsteps, h->s_guid, h->s_pooled, s));
     RF_CHECK_CUDA(cudaMemsetAsync(h->s_step, 0, sizeof(int), s));
+    // the captured step holds the LoRA scalings as kernel parameters (and skips the terms a zero scaling
+    // removes): a changed call scale is re-captured
+    if (h->graph_exec && h->graph_call_scale != h->call_scale) drop_graph(h);
     if (!h->graph_exec) {
+      h->graph_call_scale = h->call_scale;
       // capture one step: forward -> Euler update -> step counter
       cudaGraph_t graph = nullptr;
       const int64_t launches_before = rf::launch_count();

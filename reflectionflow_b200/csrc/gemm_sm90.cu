@@ -30,8 +30,9 @@ static constexpr int kMaxGroups = 3;
 struct alignas(64) GemmGroupDev {
   CUtensorMap tmA;
   CUtensorMap tmB;
-  // fused peft LoRA (groups with lora != 0, kLora kernels only): T = bf16(x A^T) [M, 64 per section] and
-  // the B factor [N, 64]; a tile in column section s = n0 / lora_sec_cols reads T columns [64 s, 64 s + 64)
+  // fused peft LoRA (groups with lora != 0, kLora kernels only): T = bf16(x A^T) [M, 64 lora per section] and
+  // the B factor [N, 64 lora]; low-rank k-block kb of a tile in column section s = n0 / lora_sec_cols reads
+  // T columns [64 (lora s + kb), +64) and B factor columns [64 kb, +64)
   CUtensorMap tmT, tmLB;
   const bf16* bias;
   bf16* out;
@@ -50,7 +51,8 @@ struct alignas(64) GemmGroupDev {
   // (s*y + ky + s-1, s*x + kx + s-1).  Tiles of the last column / row may reach past W / H: TMA zero-fills
   // the reads outside the ringed input and the epilogue skips those pixels.
   int conv_w, conv_h, conv_xt, conv_taps, conv_cin_blocks, conv_bx, conv_by, conv_stride;
-  int lora;  // this group's tiles carry the low-rank k-block (tmT, tmLB, lora_sec_cols)
+  int lora;  // this group's tiles carry `lora` (1 or 2) low-rank k-blocks (tmT, tmLB, lora_sec_cols)
+  float lora_scale[3];  // per column section: L -> bf16(bf16(L) * scale); EPI_SCALE: output scale [0]
 };
 
 struct alignas(64) GemmParamsDev {
@@ -66,6 +68,11 @@ struct GemmCfg {
   static constexpr int kStages = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);  // 192 KB of ring
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
+// A LoRA tile's math warps hold the slots of all its low-rank k-blocks until the epilogue's last half; the
+// producer can only fill them if the ring has more slots than that.
+static constexpr int kMaxLoraKb = 2;
+static_assert(GemmCfg<256>::kStages > kMaxLoraKb && GemmCfg<128>::kStages > kMaxLoraKb,
+              "the ring must hold every low-rank k-block of a tile at once");
 
 struct TileCoord {
   int g, m0, n0;  // m0: first row (group-local), n0: first column
@@ -158,17 +165,18 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
         const GemmGroupDev& G = p.g[tc.g];
         PixTile pt{0, 0};
         if (G.conv_w != 0) pt = pix_tile(G, tc.m0);
-        // a LoRA group's tile carries one extra k-block after the main ones: T rows, B factor rows of the tile
-        const int kb_end = p.num_kb + ((kLora && G.lora) ? 1 : 0);
+        // a LoRA group's tile carries G.lora extra k-blocks after the main ones: T rows, B factor rows of the tile
+        const int kb_end = p.num_kb + (kLora ? G.lora : 0);
         for (int kb = 0; kb < kb_end; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kStageBytesA;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          if (kLora && kb == p.num_kb) {
-            const int tcol = G.lora_sec_cols > 0 ? (tc.n0 / G.lora_sec_cols) * 64 : 0;
+          if (kLora && kb >= p.num_kb) {
+            const int lk = 64 * (kb - p.num_kb);
+            const int tcol = (G.lora_sec_cols > 0 ? (tc.n0 / G.lora_sec_cols) * 64 * G.lora : 0) + lk;
             tma_load_2d(sa, &G.tmT, &full_bar[stage], tcol, tc.m0);
-            tma_load_2d(sb, &G.tmLB, &full_bar[stage], 0, tc.n0);
+            tma_load_2d(sb, &G.tmLB, &full_bar[stage], lk, tc.n0);
           } else {
             if (G.conv_w != 0) {
               const int tap = kb / G.conv_cin_blocks;
@@ -232,31 +240,46 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
     fence_regs(acc);
     if (prev >= 0) release(prev);
 
-    // A LoRA group's tile: the low-rank k-block (T rows, B factor rows) follows in the ring.  It is multiplied
-    // one 128-column half at a time, right before that half's epilogue, so only a 64-register accumulator sits
-    // beside the main one; its slot is released after the last half.
+    // A LoRA group's tile: its G.lora low-rank k-blocks (T rows, B factor rows) follow in the ring.  They are
+    // multiplied one 128-column half at a time, right before that half's epilogue, so only a 64-register
+    // accumulator sits beside the main one; their slots are released after the last half.
     const bool lora = kLora && G.lora;
     const int lstage = stage;
     if (lora) {
-      mbar_wait(&full_bar[stage], phase);
-      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      for (int lk = 0; lk < G.lora; ++lk) {
+        mbar_wait(&full_bar[stage], phase);
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
     }
-    uint32_t lpk[kLora ? 32 : 1];  // bf16(L) of the current half, packed pairs in accumulator order
-    auto lora_half = [&](int hc) {
+    // the scaling of the tile's column section (a tile never straddles one: see gemm_launch)
+    const float lscale = lora ? G.lora_scale[G.lora_sec_cols > 0 ? tc.n0 / G.lora_sec_cols : 0] : 1.f;
+    uint32_t lpk[kLora ? 32 : 1];  // bf16(bf16(L) * scale) of the current half, packed pairs in accumulator order
+    auto lora_half = [&](int hc, float scale) {
       if constexpr (kLora) {
         float accl[64];
 #pragma unroll
         for (int i = 0; i < 64; ++i) accl[i] = 0.f;
+        auto slot = [&](int lk) { return lstage + lk < Cfg::kStages ? lstage + lk : lstage + lk - Cfg::kStages; };
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k)  // B rows [128 hc, 128 hc + 128): + hc * 16 KB (encoded >> 4)
-          wgmma_ss_n128(accl, a_desc(lstage) + 2 * k, b_desc(lstage) + hc * 1024 + 2 * k, k != 0);
+        for (int lk = 0; lk < kMaxLoraKb; ++lk) {
+          if (lk < G.lora) {
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)  // B rows [128 hc, 128 hc + 128): + hc * 16 KB (encoded >> 4)
+              wgmma_ss_n128(accl, a_desc(slot(lk)) + 2 * k, b_desc(slot(lk)) + hc * 1024 + 2 * k, (lk | k) != 0);
+          }
+        }
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(accl);
-        if (hc == BN / 128 - 1) release(lstage);
+        if (hc == BN / 128 - 1)
+          for (int lk = 0; lk < G.lora; ++lk) release(slot(lk));
 #pragma unroll
-        for (int i = 0; i < 32; ++i) lpk[i] = pack_bf16x2(accl[2 * i], accl[2 * i + 1]);
+        for (int i = 0; i < 32; ++i) {
+          float l0 = accl[2 * i], l1 = accl[2 * i + 1];
+          bf16_round2(l0, l1);  // peft: bf16(T B^T) * scaling, in fp32, rounded to bf16 at the pack
+          lpk[i] = pack_bf16x2(__fmul_rn(l0, scale), __fmul_rn(l1, scale));
+        }
       }
     };
 
@@ -319,7 +342,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
       for (int hc = 0; hc < BN / 128; ++hc) {
         const int col_h = tc.n0 + hc * 128;
         const int section = col_h / inner;  // 0 q, 1 k, 2 v
-        if (lora) lora_half(hc);
+        if (lora) lora_half(hc, lscale);
         float v[2][32];
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj)
@@ -364,7 +387,7 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = tc.n0 + 8 * j + cq;
-        if (lora && j % 16 == 0) lora_half(j / 16);
+        if (lora && j % 16 == 0) lora_half(j / 16, lscale);
 #pragma unroll
         for (int h2 = 0; h2 < 2; ++h2) {
           float v0, v1;
@@ -372,6 +395,10 @@ gemm_kernel(const __grid_constant__ GemmParamsDev p) {
           if constexpr (EPI == EPI_GELU) {
             v0 = gelu_tanh(v0);
             v1 = gelu_tanh(v1);
+          }
+          if constexpr (EPI == EPI_SCALE) {
+            v0 = __fmul_rn(v0, G.lora_scale[0]);
+            v1 = __fmul_rn(v1, G.lora_scale[0]);
           }
           if constexpr (EPI == EPI_GATE_RES) {
             if (ok[h2]) {
@@ -488,6 +515,8 @@ int gemm_init() {
   rc |= set_attr<128, EPI_GATE_RES, false>(); rc |= set_attr<128, EPI_QKV, false>();
   rc |= set_attr<64, EPI_BIAS, false>(); rc |= set_attr<64, EPI_GELU, false>();
   rc |= set_attr<64, EPI_GATE_RES, false>();
+  rc |= set_attr<256, EPI_SCALE, false>(); rc |= set_attr<128, EPI_SCALE, false>();
+  rc |= set_attr<64, EPI_SCALE, false>();
   rc |= set_attr<256, EPI_GELU, true>(); rc |= set_attr<256, EPI_GATE_RES, true>();
   rc |= set_attr<256, EPI_QKV, true>();
   rc |= set_attr<128, EPI_GELU, true>(); rc |= set_attr<128, EPI_GATE_RES, true>();
@@ -508,7 +537,7 @@ static int launch_cfg(GemmParamsDev& p, const char* name, cudaStream_t stream) {
   const int grid = grid_ctas(p.total_tiles);
   double rows = 0;
   for (int g = 0; g < p.ngroups; ++g) rows += p.g[g].M;
-  static const char* kNames[4] = {"gemm_bias", "gemm_gelu", "gemm_gate_res", "gemm_qkv_rms_rope"};
+  static const char* kNames[5] = {"gemm_bias", "gemm_gelu", "gemm_gate_res", "gemm_qkv_rms_rope", "gemm_scale"};
   const bool conv = p.g[0].conv_w != 0;
   if (name == nullptr) name = conv ? (EPI == EPI_GATE_RES ? "conv_res" : "conv_bias") : kNames[EPI];
   // algorithmic FLOPs: 2 M N K; algorithmic bytes: A (each pixel once for a convolution) + W + out once
@@ -539,6 +568,7 @@ static int launch_bn(int epi, GemmParamsDev& p, const char* name, cudaStream_t s
       case EPI_QKV:
         if constexpr (BN >= 128) return launch_cfg<BN, EPI_QKV, false>(p, name, stream);
         break;
+      case EPI_SCALE: return launch_cfg<BN, EPI_SCALE, false>(p, name, stream);
       default: break;
     }
   }
@@ -586,10 +616,15 @@ static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupA
     const GemmGroupArgs& a = groups[g];
     if (a.lora_T == nullptr) continue;
     if (a.lora_B == nullptr || !gemm_lora_eligible(epi, N, K, a) ||
-        (a.lora_sec_cols > 0 && (a.lora_sec_cols % 128 != 0 || N % a.lora_sec_cols != 0))) {
+        (a.lora_sec_cols > 0 && (a.lora_sec_cols % 128 != 0 || N % a.lora_sec_cols != 0 || N / a.lora_sec_cols > 3))) {
       set_error("gemm_launch: LoRA group needs M >= 128, N % 128 == 0 (QKV: N % 384 == 0), 16-byte aligned "
-                "out / res pitches, no addend, sections of a multiple of 128 columns, and the GELU / GATE_RES / "
-                "QKV epilogue");
+                "out / res pitches, no addend, at most 3 sections of a multiple of 128 columns, and the GELU / "
+                "GATE_RES / QKV epilogue");
+      return -1;
+    }
+    // the math warps hold every low-rank k-block's ring slot at once (static_assert on GemmCfg above)
+    if (a.lora_pad != 64 && a.lora_pad != 64 * kMaxLoraKb) {
+      set_error("gemm_launch: lora_pad must be 64 or 128");
       return -1;
     }
     // a tile reads the T columns of one section: 256-wide tiles only when they cannot straddle one
@@ -627,14 +662,15 @@ static int gemm_launch_impl(int epi, int N, int K, int ngroups, const GemmGroupA
     rc = make_tmap_2d(&d.tmB, a.W, N, K, K, bn);
     if (rc) return rc;
     if (a.lora_T != nullptr) {
-      const int t_cols = a.lora_sec_cols > 0 ? (N / a.lora_sec_cols) * 64 : 64;
+      const int t_cols = a.lora_sec_cols > 0 ? (N / a.lora_sec_cols) * a.lora_pad : a.lora_pad;
       rc = make_tmap_2d(&d.tmT, a.lora_T, a.M, t_cols, a.ld_t, BM);
       if (rc) return rc;
-      rc = make_tmap_2d(&d.tmLB, a.lora_B, N, 64, 64, bn);
+      rc = make_tmap_2d(&d.tmLB, a.lora_B, N, a.lora_pad, a.lora_pad, bn);
       if (rc) return rc;
-      d.lora = 1;
+      d.lora = a.lora_pad / 64;
       d.lora_sec_cols = a.lora_sec_cols;
     }
+    for (int s = 0; s < 3; ++s) d.lora_scale[s] = a.lora_scale[s];
     d.bias = a.bias; d.out = a.out; d.addend = a.addend; d.res = a.res; d.gate = a.gate;
     d.rope_cos = a.rope_cos; d.rope_sin = a.rope_sin; d.norm_q = a.norm_q; d.norm_k = a.norm_k;
     d.M = a.M; d.ldo = a.ldo; d.ldadd = a.ldadd; d.ldr = a.ldr;

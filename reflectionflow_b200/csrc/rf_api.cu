@@ -175,6 +175,8 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
   g.lora_T = T; g.ld_t = t_cols;
   g.lora_B = static_cast<const bf16*>(lora_B);
   g.lora_sec_cols = t_cols == 192 ? N / 3 : 0;
+  g.lora_pad = 64;
+  g.lora_scale[0] = g.lora_scale[1] = g.lora_scale[2] = 1.f;
   return rf::gemm_launch(epilogue, N, K, 1, &g, s);
 }
 

@@ -74,6 +74,7 @@ enum GemmEpilogue {
   EPI_GELU = 1,      // out = bf16(gelu_tanh(bf16(acc + bias)))
   EPI_GATE_RES = 2,  // out = bf16(res + bf16(gate[n] * bf16(acc + bias)))
   EPI_QKV = 3,       // q,k sections: per-head RMSNorm * w, interleaved RoPE; v: bias only
+  EPI_SCALE = 4,     // out = bf16(bf16(acc + bias) * lora_scale[0]): peft's scaled low-rank term, unfused
 };
 
 // One member of a grouped GEMM: out[M, N] = epi(A[M, K] @ W[N, K]^T).  All groups of a
@@ -91,12 +92,18 @@ struct GemmGroupArgs {
   const bf16* norm_q;              // EPI_QKV: [128]
   const bf16* norm_k;
   // peft's unfused LoRA arithmetic fused into this group's tiles (lora_T != nullptr):
-  //   out = epi( bf16( bf16(A W^T + b) + bf16(T lora_B^T) ) ),  T = bf16(A loraA^T) computed beforehand.
+  //   out = epi( bf16( bf16(A W^T + b) + bf16( bf16(T lora_B^T) * lora_scale[s] ) ) ),
+  //   T = bf16(A loraA^T) computed beforehand.
   // T: [M, ld_t]; with lora_sec_cols > 0 output section s = n / lora_sec_cols reads T columns
-  // [64 s, 64 s + 64) (stacked q|k|v); lora_B: [N, 64] (rank zero-padded to 64).  See gemm_lora_eligible.
+  // [lora_pad s, lora_pad (s + 1)) (stacked q|k|v), else s = 0 and T columns [0, lora_pad); lora_B: [N, lora_pad]
+  // (rank zero-padded to lora_pad = 64 or 128: one or two 64-deep low-rank k-blocks).  lora_scale[s] is the
+  // fp32 peft scaling of section s (1: the multiply is the identity).  See gemm_lora_eligible.
+  // EPI_SCALE reads lora_scale[0] as its output scale.
   const bf16* lora_T; int ld_t;
   const bf16* lora_B;
   int lora_sec_cols;
+  int lora_pad;
+  float lora_scale[3];
 };
 int gemm_launch(int epi, int N, int K, int ngroups, const GemmGroupArgs* groups,
                 cudaStream_t stream);
@@ -157,7 +164,8 @@ int euler_step_launch(bf16* x, const bf16* v, const float* sigmas, const int* st
                       cudaStream_t stream);
 int copy_rows_launch(const bf16* src, int lds, bf16* dst, int ldd, int rows, int cols,
                      cudaStream_t stream);
-// dst[r * ldd + c] = bf16(dst[r * ldd + c] + src[r * lds + c]) for r < rows, c < cols
-int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, cudaStream_t stream);
+// dst[r * ldd + c] = bf16(dst[r * ldd + c] + bf16(src[r * lds + c] * scale)) for r < rows, c < cols
+int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, float scale,
+                    cudaStream_t stream);
 
 }  // namespace rf

@@ -17,6 +17,7 @@ through a user-supplied `text_encoder_hook`) and `output_type` must be "latent".
 """
 from __future__ import annotations
 
+import os
 from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Any, Callable, Dict, List, Optional, Union
@@ -26,7 +27,7 @@ import torch
 
 from .config import FluxDiTConfig
 from .scheduler import FlowMatchEulerDiscreteScheduler, calculate_shift
-from .transformer import B200FluxTransformer2DModel
+from .transformer import B200FluxTransformer2DModel, lora_scale
 
 # train_flux/flux/condition.py:10-21.  The tts path uses "cot"; the DiT treats every type alike (the type-id column is
 # produced but not consumed, transformer.py:133), so the other types only differ in how `raw_img` becomes the condition.
@@ -160,9 +161,12 @@ class B200FluxPipeline:
 
     def load_lora_weights(self, lora, adapter_name: str = "reflection", alpha: Optional[float] = None):
         """pipe.load_lora_weights(lora_path, adapter_name=...) (tts_reflectionflow.py:503-505):
-        `lora` is a state dict / {module: (A, B)} mapping or a .safetensors path."""
-        if isinstance(lora, str):
+        `lora` is a state dict / {module: (A, B)} mapping, a .safetensors path, or a directory holding
+        pytorch_lora_weights.safetensors (what train_flux's save_lora writes, train/model.py:87-92)."""
+        if isinstance(lora, (str, os.PathLike)):
             from safetensors.torch import load_file
+            if os.path.isdir(lora):
+                lora = os.path.join(lora, "pytorch_lora_weights.safetensors")
             lora = load_file(lora)
         self.transformer.load_lora(lora, alpha)
 
@@ -477,8 +481,10 @@ def generate(pipeline: B200FluxPipeline, conditions: List[Condition] = None, con
             ids.append(i)
         cond_lat = torch.cat(toks, dim=1)
         cond_ids = torch.cat(ids, dim=0)
-    latents = self._denoise(latents, prompt_embeds, pooled_prompt_embeds, text_ids, latent_image_ids,
-                            num_inference_steps, guidance_scale, params.get("timesteps"), cond_lat,
-                            cond_ids, model_config, condition_scale)
+    # joint_attention_kwargs["scale"] reaches every step of the loop (generate.py:246 -> transformer.py:73-81)
+    with lora_scale(self.transformer, self._joint_attention_kwargs):
+        latents = self._denoise(latents, prompt_embeds, pooled_prompt_embeds, text_ids, latent_image_ids,
+                                num_inference_steps, guidance_scale, params.get("timesteps"), cond_lat,
+                                cond_ids, model_config, condition_scale)
     return self._finish(latents, height, width, params.get("output_type", "pil"),
                         params.get("return_dict", True))

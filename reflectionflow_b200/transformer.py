@@ -13,6 +13,7 @@ kernels.  There is no PyTorch fallback: without librf_b200.so or without a GPU t
 from __future__ import annotations
 
 import ctypes
+from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Any, Dict, Optional
 
@@ -42,10 +43,40 @@ def _bf16c(t: torch.Tensor, device) -> torch.Tensor:
     return t.detach().to(device=device, dtype=torch.bfloat16).contiguous()
 
 
+MAX_LORA_RANK = 128
+
+
+def _lora_pairs(lora: Dict[str, Any], max_rank: int) -> Dict[str, Any]:
+    """{module_path: (A [r, in], B [out, r])} from either that mapping or a peft / diffusers LoRA state dict with
+    keys `[transformer.]<module>.lora_A.weight` / `.lora_B.weight`; refuses factors that are not [r, in] / [out, r]
+    and ranks above `max_rank`."""
+    if lora and all(isinstance(v, (tuple, list)) for v in lora.values()):
+        pairs = dict(lora)
+    else:
+        tmp: Dict[str, Dict[str, torch.Tensor]] = {}
+        for k, v in lora.items():
+            k = k[len("transformer."):] if k.startswith("transformer.") else k
+            for tag in (".lora_A", ".lora_B"):
+                if tag in k:
+                    mod = k.split(tag)[0]
+                    tmp.setdefault(mod, {})[tag] = v
+        pairs = {m: (d[".lora_A"], d[".lora_B"]) for m, d in tmp.items()}
+    for mod, (A, B) in pairs.items():
+        if A.ndim != 2 or B.ndim != 2 or B.shape[1] != A.shape[0]:
+            raise ValueError(f"LoRA factors of {mod}: A {tuple(A.shape)} / B {tuple(B.shape)} "
+                             "are not [r, in] / [out, r]")
+        if A.shape[0] > max_rank:
+            raise ValueError(f"LoRA rank {A.shape[0]} of {mod} exceeds the model's lora_rank {max_rank}: "
+                             f"create the model with lora_rank >= {A.shape[0]} (at most {MAX_LORA_RANK})")
+    return pairs
+
+
 class B200FluxTransformer2DModel:
     """Owns one rf_dit handle (weights resident in HBM, packed for the kernels)."""
 
     def __init__(self, config=None, lora_rank: int = 0, device="cuda:0"):
+        if not 0 <= int(lora_rank) <= MAX_LORA_RANK:
+            raise ValueError(f"lora_rank must be 0..{MAX_LORA_RANK}, got {lora_rank}")
         if not torch.cuda.is_available():
             raise L.RFError("B200FluxTransformer2DModel needs a CUDA device; there is no CPU fallback")
         self.cfg = FluxDiTConfig.from_any(config or FluxDiTConfig())
@@ -63,6 +94,7 @@ class B200FluxTransformer2DModel:
         # "merged": condition tokens use W + BA (peft fuse_lora; the reference leaves that call
         # commented out at tts_reflectionflow.py:506) — no extra kernels, +11.5 GB of weights.
         self.lora_mode = "exact"
+        self.has_lora = False  # an adapter is loaded: the call-level LoRA scale has something to act on
         with torch.cuda.device(self.device):
             c = _RfDitConfig(self.cfg.num_layers, self.cfg.num_single_layers,
                              self.cfg.num_attention_heads, self.cfg.in_channels,
@@ -167,40 +199,34 @@ class B200FluxTransformer2DModel:
 
     def load_lora(self, lora: Dict[str, Any], alpha: Optional[float] = None, mode: Optional[str] = None):
         """`lora`: {module_path: (A [r,in], B [out,r])}  or a peft/diffusers LoRA state dict with
-        keys `[transformer.]<module>.lora_A.weight` / `.lora_B.weight`.  scaling = alpha / r
-        (train_flux/config.yaml:50-51: r = alpha = 32 -> 1)."""
+        keys `[transformer.]<module>.lora_A.weight` / `.lora_B.weight`.  scaling = alpha / r per module, r
+        taken from that module's factors (alpha None: scaling 1; train_flux/config.yaml:50-51 r = alpha = 32).
+        Ranks up to the model's lora_rank (<= 128)."""
         if self.lora_rank <= 0:
             raise L.RFError("model was created with lora_rank=0")
         if mode is not None:
             if mode not in ("exact", "merged"):
                 raise ValueError("lora mode must be 'exact' or 'merged'")
             self.lora_mode = mode
+        pairs = _lora_pairs(lora, self.lora_rank)
         self._geom_key = None  # adapters changed: rf_dit_prepare must re-run (merged copies, graph)
-        pairs = {}
-        if lora and all(isinstance(v, (tuple, list)) for v in lora.values()):
-            pairs = dict(lora)
-        else:
-            tmp: Dict[str, Dict[str, torch.Tensor]] = {}
-            for k, v in lora.items():
-                k = k[len("transformer."):] if k.startswith("transformer.") else k
-                for tag in (".lora_A", ".lora_B"):
-                    if tag in k:
-                        mod = k.split(tag)[0]
-                        tmp.setdefault(mod, {})[tag] = v
-            pairs = {m: (d[".lora_A"], d[".lora_B"]) for m, d in tmp.items()}
         with torch.cuda.device(self.device):
             for mod, (A, B) in pairs.items():
                 r = A.shape[0]
-                if A.ndim != 2 or B.ndim != 2 or B.shape[1] != r:
-                    raise ValueError(f"LoRA factors of {mod}: A {tuple(A.shape)} / B {tuple(B.shape)} "
-                                     "are not [r, in] / [out, r]")
                 scale = 1.0 if alpha is None else float(alpha) / r
                 a, b = _bf16c(A, self.device), _bf16c(B, self.device)
                 L.check(self._lib.rf_dit_set_lora(self._h, mod.encode(), L.ptr(a), L.ptr(b), r,
                                                   int(A.shape[1]), int(B.shape[0]),
                                                   ctypes.c_float(scale)), f"rf_dit_set_lora({mod})")
+                self.has_lora = True
             torch.cuda.synchronize(self.device)
         return self
+
+    def set_lora_scale(self, scale: float):
+        """diffusers' LoRA strength (joint_attention_kwargs["scale"]): multiplies every adapter's alpha / r from
+        the next call on, until set again (1 = as loaded).  A captured denoise step built for another scale is
+        re-captured, merged weights are re-merged."""
+        L.check(self._lib.rf_dit_set_lora_scale(self._h, ctypes.c_double(float(scale))), "rf_dit_set_lora_scale")
 
     # ------------------------------------------------------------------ geometry
     def _flags(self, model_config: Optional[Dict[str, Any]]) -> int:
@@ -301,6 +327,24 @@ class B200FluxTransformer2DModel:
         return lat
 
 
+@contextmanager
+def lora_scale(transformer, joint_attention_kwargs: Optional[Dict[str, Any]]):
+    """joint_attention_kwargs["scale"] for one call: diffusers' scale_lora_layers before it, unscale after
+    (train_flux/flux/transformer.py:73-81,248).  Without a scale (or with 1) the transformer is not touched.  A
+    scale other than 1 needs a loaded adapter: without one it could have no effect, so it is refused."""
+    s = 1.0 if joint_attention_kwargs is None else joint_attention_kwargs.get("scale", 1.0)
+    if s is None or s == 1.0:
+        yield
+        return
+    if not getattr(transformer, "has_lora", False):
+        raise NotImplementedError("joint_attention_kwargs['scale'] != 1 scales a LoRA adapter, and none is loaded")
+    transformer.set_lora_scale(float(s))
+    try:
+        yield
+    finally:
+        transformer.set_lora_scale(1.0)
+
+
 def tranformer_forward(transformer: B200FluxTransformer2DModel, condition_latents, condition_ids,
                        condition_type_ids, model_config: Optional[Dict[str, Any]] = {}, c_t=0,
                        **params):
@@ -308,17 +352,15 @@ def tranformer_forward(transformer: B200FluxTransformer2DModel, condition_latent
     train_flux/flux/transformer.py:47-55,250-252."""
     if c_t != 0:
         raise NotImplementedError("c_t != 0 is never used by the reference's callers")
-    jak = params.get("joint_attention_kwargs")
-    if jak is not None and jak.get("scale", 1.0) != 1.0:
-        raise NotImplementedError("joint_attention_kwargs['scale'] != 1 is not supported")
     if params.get("controlnet_block_samples") is not None or \
             params.get("controlnet_single_block_samples") is not None:
         raise NotImplementedError("controlnet residuals (transformer.py:26-27,182,226) are not on the tts path")
     cscale = float(getattr(transformer, "condition_scale", 1.0))
-    out = transformer._forward(params["hidden_states"], params.get("encoder_hidden_states"),
-                               params.get("pooled_projections"), params.get("timestep"),
-                               params.get("img_ids"), params.get("txt_ids"), params.get("guidance"),
-                               condition_latents, condition_ids, model_config or {}, cscale)
+    with lora_scale(transformer, params.get("joint_attention_kwargs")):
+        out = transformer._forward(params["hidden_states"], params.get("encoder_hidden_states"),
+                                   params.get("pooled_projections"), params.get("timestep"),
+                                   params.get("img_ids"), params.get("txt_ids"), params.get("guidance"),
+                                   condition_latents, condition_ids, model_config or {}, cscale)
     if not params.get("return_dict", True):
         return (out,)
     return Transformer2DModelOutput(sample=out)
