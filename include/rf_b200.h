@@ -137,20 +137,37 @@ void rf_dit_destroy(rf_dit* h);
  * DiffusionPipeline.from_pretrained(...).to("cuda") (tts/tts_reflectionflow.py:498-501). */
 int rf_dit_load_weight(rf_dit* h, const char* key, const void* src, int64_t numel);
 
-/* peft LoRA factors of one target Linear (pipe.load_lora_weights, tts_reflectionflow.py:503-505;
- * target list train_flux/config.yaml:53).  module = diffusers module path without ".weight"
- * (e.g. "single_transformer_blocks.0.proj_out"); A: [r, in_features] bf16, B: [out_features, r]
- * bf16 (device); in_/out_features are checked against the target Linear (a mismatched adapter
- * file is an error, not an out-of-bounds read); r <= lora_rank; scale = that target's lora_alpha / r,
- * any finite value (NaN / inf are refused).  Applied to condition tokens only unless latent_lora is set in
- * rf_dit_prepare (lora_controller.py:5-42); with it, to every token that passes the target: the image stream
- * of the double blocks, the txt + img rows of the single blocks, and the image / main-row adaLN modulation
- * (norm1.linear / norm.linear of temb).
+/* peft LoRA factors of one target Linear (pipe.load_lora_weights, tts_reflectionflow.py:503-505).  Any Linear of
+ * FluxTransformer2DModel is a target (train/model.py:73-80 "all-linear"); other parameters (norm_q, biases, ...) are
+ * refused.  module = diffusers module path without ".weight" (e.g. "single_transformer_blocks.0.proj_out");
+ * A: [r, in_features] bf16, B: [out_features, r] bf16 (device); in_/out_features are checked against the target
+ * Linear (a mismatched adapter file is an error, not an out-of-bounds read); r <= lora_rank; scale = that target's
+ * lora_alpha / r, any finite value (NaN / inf are refused).  Setting a target again replaces its factors; targets
+ * stay set until rf_dit_clear_lora.
+ * Which rows carry the term follows lora_controller.py:5-42 (enable_lora zeroes the scaling of the modules it
+ * names, inside its block only):
+ *   x_embedder, and per block norm1.linear, attn.to_q/to_k/to_v, attn.to_out.0, ff.net.2 (double) and norm.linear,
+ *   attn.to_q/to_k/to_v, proj_mlp, proj_out (single): the condition tokens (and cond_temb's modulation); with
+ *   latent_lora (rf_dit_prepare) also the image stream of the double blocks, the txt + img rows of the single
+ *   blocks and the image / main-row modulation of temb;
+ *   context_embedder: the text rows, always;
+ *   time_text_embed.{timestep,guidance,text}_embedder.linear_{1,2}: temb and cond_temb, always (every modulation
+ *   vector downstream changes);
+ *   norm_out.linear: the final modulation, always;  proj_out (top level): the image rows, always;
+ *   per double block norm1_context.linear, attn.add_q_proj/add_k_proj/add_v_proj (before norm_added_q/k and RoPE),
+ *   attn.to_add_out, ff_context.net.0.proj (before the GELU), ff_context.net.2: the text stream, always;
+ *   per double block ff.net.0.proj (before the GELU): the image rows always and the condition rows.
+ * The factors of the Linears outside train_flux/config.yaml:53 are allocated on their first rf_dit_set_lora.
  * Arithmetic (peft): y = bf16( bf16(x W^T + b) + bf16( bf16(T B^T) * s ) ), T = bf16(x A^T), with s the
  * target's effective scaling float(scale * call_scale) (product in double, as peft's `scaling *= scale`;
  * call_scale from rf_dit_set_lora_scale).  A target whose s is 0 adds nothing and runs no launch. */
 int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B, int r,
                     int in_features, int out_features, float scale);
+
+/* Unset every LoRA target (diffusers' unload_lora_weights): the handle computes the adapter-free model until
+ * rf_dit_set_lora is called again.  The factor storage stays allocated (zeroed); merged copies are re-made and the
+ * captured denoise step is re-captured at the next call. */
+int rf_dit_clear_lora(rf_dit* h);
 
 /* The call-level LoRA multiplier (diffusers' joint_attention_kwargs["scale"], scale_lora_layers): every
  * target's scaling is multiplied by `scale` from the next rf_dit_forward / rf_dit_denoise on; 1 by default,

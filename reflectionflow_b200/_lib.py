@@ -88,6 +88,8 @@ def _declare(lib):
         lib.rf_dit_set_lora.argtypes = [vp, c_char_p, vp, vp, ci, ci, ci, cf]
         lib.rf_dit_set_lora_scale.restype = ci
         lib.rf_dit_set_lora_scale.argtypes = [vp, ctypes.c_double]
+        lib.rf_dit_clear_lora.restype = ci
+        lib.rf_dit_clear_lora.argtypes = [vp]
         lib.rf_dit_missing_weights.restype = ci
         lib.rf_dit_missing_weights.argtypes = [vp]
         lib.rf_dit_prepare.restype = ci

@@ -41,6 +41,12 @@ int gemv_init();
 
 using rf::bf16;
 
+#define RF_TRY(expr)            \
+  do {                          \
+    int _rc = (expr);           \
+    if (_rc != 0) return _rc;   \
+  } while (0)
+
 namespace {
 
 struct Slot {
@@ -60,6 +66,15 @@ struct LoraT {  // factors of one target, rank zero-padded to the handle's lora_
   int in = 0, out = 0;
   bool set = false;
   double scale = 1.0;  // lora_alpha / r
+  // The Linears outside train_flux/config.yaml:53 (text stream, embedders, final layer, ff.net.0.proj) are "always"
+  // targets: no enable_lora block names them, so every call applies them, latent_lora or not.  Their factors are
+  // allocated on the first rf_dit_set_lora, so a handle that never sees such an adapter keeps its footprint.  A
+  // member of a stacked pack (add_q|k|v) allocates the whole pack, zeroed, and points its siblings into it.
+  bool always = false;
+  LoraT* pack[3] = {nullptr, nullptr, nullptr};
+  int npack = 0;
+  bf16** packA = nullptr;
+  bf16** packB = nullptr;
 };
 // (merged weights W + B A of a whole packed projection live in the block structs: *_m)
 
@@ -67,9 +82,14 @@ struct DoubleBlk {
   Lin qkv, add_qkv, to_out, to_add_out, ff1, ff2, ffc1, ffc2;
   bf16 *norm_q, *norm_k, *norm_added_q, *norm_added_k;
   LoraT l_norm1, l_q, l_k, l_v, l_out, l_ff2;
+  // always targets: text stream (norm1_context, add_q|k|v, to_add_out, ff_context) and ff.net.0.proj
+  LoraT l_norm1c, l_aq, l_ak, l_av, l_add_out, l_ff1, l_ffc1, l_ffc2;
   bf16* qkvA = nullptr;  // [3 lora_pad, D] = stacked A of to_q/to_k/to_v
   bf16* qkvB = nullptr;  // [3D, lora_pad] = stacked B (rows of the packed q|k|v projection)
+  bf16* add_qkvA = nullptr;  // the same for add_q_proj / add_k_proj / add_v_proj (allocated on first use)
+  bf16* add_qkvB = nullptr;
   bf16 *qkv_m = nullptr, *to_out_m = nullptr, *ff2_m = nullptr;  // merged W + B A (fuse_lora mode)
+  bf16 *add_qkv_m = nullptr, *to_add_out_m = nullptr, *ff1_m = nullptr, *ffc1_m = nullptr, *ffc2_m = nullptr;
 };
 struct SingleBlk {
   Lin qkv, mlp, out;
@@ -93,12 +113,15 @@ struct rf_dit {
   std::unordered_map<std::string, LoraT*> lora_slots;
   Lin x_emb, ctx_emb, t1, t2, g1, g2, p1, p2, proj_out;
   LoraT l_x_emb;
+  // always targets at the top level: context_embedder, the time / guidance / text embedders, norm_out, proj_out
+  LoraT l_ctx, l_t1, l_t2, l_g1, l_g2, l_p1, l_p2, l_norm_out, l_proj_out;
   bf16* modW = nullptr;
   bf16* modB = nullptr;
   int64_t n_mod = 0;
   std::vector<DoubleBlk> dbl;
   std::vector<SingleBlk> sgl;
   bool any_lora = false;
+  bool any_always = false;  // some always target is set: its rows carry a LoRA whatever the flags
   // LoRA rank padding: 64 for lora_rank <= 64, else 128 (one or two 64-deep low-rank k-blocks per fused tile)
   int lora_pad = 64;
   // rf_dit_set_lora_scale: peft's call-level multiplier (joint_attention_kwargs["scale"]); a target's effective
@@ -108,6 +131,7 @@ struct rf_dit {
   double merged_call_scale = 1.0;
   bool use_merged = false;    // rf_dit_prepare flag bit 3
   bf16* x_emb_m = nullptr;
+  bf16 *ctx_emb_m = nullptr, *proj_out_m = nullptr;
   // ---- geometry
   bool prepared = false;
   int batch = 0, n_txt = 0, n_img = 0, n_cond = 0, N = 0, n_main = 0;
@@ -192,6 +216,40 @@ void new_lora(rf_dit* h, Arena& ar, const std::string& mod, LoraT& t, int out, i
   h->lora_slots[mod] = &t;
 }
 
+// an always target: shape checks now, factor storage on its first rf_dit_set_lora (lora_storage)
+void new_always_lora(rf_dit* h, const std::string& mod, LoraT& t, int out, int in) {
+  if (h->cfg.lora_rank <= 0) return;
+  t.in = in;
+  t.out = out;
+  t.always = true;
+  h->lora_slots[mod] = &t;
+}
+
+// zeroed factor storage of target t (of its whole pack), allocated on first use; live until destroy
+int lora_storage(rf_dit* h, LoraT& t) {
+  if (t.A != nullptr) return 0;
+  const int64_t pad = h->lora_pad, n = t.npack ? t.npack : 1;
+  const int64_t a_elems = pad * t.in, b_elems = static_cast<int64_t>(t.out) * pad;
+  void *pa = nullptr, *pb = nullptr;
+  RF_TRY(dev_alloc(h, &pa, static_cast<size_t>(n * a_elems) * 2));
+  RF_TRY(dev_alloc(h, &pb, static_cast<size_t>(n * b_elems) * 2));
+  RF_CHECK_CUDA(cudaMemset(pa, 0, static_cast<size_t>(n * a_elems) * 2));
+  RF_CHECK_CUDA(cudaMemset(pb, 0, static_cast<size_t>(n * b_elems) * 2));
+  bf16 *A = static_cast<bf16*>(pa), *B = static_cast<bf16*>(pb);
+  if (t.npack == 0) {
+    t.A = A;
+    t.B = B;
+    return 0;
+  }
+  *t.packA = A;
+  *t.packB = B;
+  for (int k = 0; k < t.npack; ++k) {
+    t.pack[k]->A = A + k * a_elems;
+    t.pack[k]->B = B + k * b_elems;
+  }
+  return 0;
+}
+
 int build_storage(rf_dit* h) {
   const rf_dit_config& c = h->cfg;
   const int D = h->D, lpad = h->lora_pad;
@@ -199,15 +257,24 @@ int build_storage(rf_dit* h) {
   h->x_emb = new_lin(h, ar, "x_embedder", D, c.in_channels);
   new_lora(h, ar, "x_embedder", h->l_x_emb, D, c.in_channels);
   h->ctx_emb = new_lin(h, ar, "context_embedder", D, c.joint_attention_dim);
-  h->t1 = new_lin(h, ar, "time_text_embed.timestep_embedder.linear_1", D, 256);
-  h->t2 = new_lin(h, ar, "time_text_embed.timestep_embedder.linear_2", D, D);
+  new_always_lora(h, "context_embedder", h->l_ctx, D, c.joint_attention_dim);
+  const std::string tte = "time_text_embed.";
+  h->t1 = new_lin(h, ar, tte + "timestep_embedder.linear_1", D, 256);
+  h->t2 = new_lin(h, ar, tte + "timestep_embedder.linear_2", D, D);
+  new_always_lora(h, tte + "timestep_embedder.linear_1", h->l_t1, D, 256);
+  new_always_lora(h, tte + "timestep_embedder.linear_2", h->l_t2, D, D);
   if (c.guidance_embeds) {
-    h->g1 = new_lin(h, ar, "time_text_embed.guidance_embedder.linear_1", D, 256);
-    h->g2 = new_lin(h, ar, "time_text_embed.guidance_embedder.linear_2", D, D);
+    h->g1 = new_lin(h, ar, tte + "guidance_embedder.linear_1", D, 256);
+    h->g2 = new_lin(h, ar, tte + "guidance_embedder.linear_2", D, D);
+    new_always_lora(h, tte + "guidance_embedder.linear_1", h->l_g1, D, 256);
+    new_always_lora(h, tte + "guidance_embedder.linear_2", h->l_g2, D, D);
   }
-  h->p1 = new_lin(h, ar, "time_text_embed.text_embedder.linear_1", D, c.pooled_projection_dim);
-  h->p2 = new_lin(h, ar, "time_text_embed.text_embedder.linear_2", D, D);
+  h->p1 = new_lin(h, ar, tte + "text_embedder.linear_1", D, c.pooled_projection_dim);
+  h->p2 = new_lin(h, ar, tte + "text_embedder.linear_2", D, D);
+  new_always_lora(h, tte + "text_embedder.linear_1", h->l_p1, D, c.pooled_projection_dim);
+  new_always_lora(h, tte + "text_embedder.linear_2", h->l_p2, D, D);
   h->proj_out = new_lin(h, ar, "proj_out", c.in_channels, D);
+  new_always_lora(h, "proj_out", h->l_proj_out, c.in_channels, D);
 
   h->n_mod = static_cast<int64_t>(c.num_layers) * 12 * D +
              static_cast<int64_t>(c.num_single_layers) * 3 * D + 2 * D;
@@ -222,6 +289,7 @@ int build_storage(rf_dit* h) {
     reg_lin(h, p + "norm1.linear", h->modW + mo * D, h->modB + mo, 6 * D, D);
     reg_lin(h, p + "norm1_context.linear", h->modW + (mo + 6 * D) * D, h->modB + mo + 6 * D, 6 * D, D);
     new_lora(h, ar, p + "norm1.linear", b.l_norm1, 6 * D, D);
+    new_always_lora(h, p + "norm1_context.linear", b.l_norm1c, 6 * D, D);
     b.qkv = new_lin(h, ar, "", 3 * D, D);
     b.add_qkv = new_lin(h, ar, "", 3 * D, D);
     const char* nm[3] = {"to_q", "to_k", "to_v"};
@@ -231,6 +299,7 @@ int build_storage(rf_dit* h) {
       b.qkvB = ar.take(static_cast<int64_t>(3 * D) * lpad);
     }
     LoraT* lq[3] = {&b.l_q, &b.l_k, &b.l_v};
+    LoraT* la[3] = {&b.l_aq, &b.l_ak, &b.l_av};
     for (int j = 0; j < 3; ++j) {
       reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
       reg_lin(h, p + "attn." + an[j], b.add_qkv.w + static_cast<int64_t>(j) * D * D,
@@ -238,6 +307,11 @@ int build_storage(rf_dit* h) {
       new_lora(h, ar, p + "attn." + nm[j], *lq[j], D, D,
                b.qkvA ? b.qkvA + static_cast<int64_t>(j) * lpad * D : nullptr,
                b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * lpad : nullptr);
+      new_always_lora(h, p + "attn." + an[j], *la[j], D, D);
+      la[j]->npack = 3;
+      la[j]->packA = &b.add_qkvA;
+      la[j]->packB = &b.add_qkvB;
+      for (int k = 0; k < 3; ++k) la[j]->pack[k] = la[k];
     }
     b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
     b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
@@ -246,11 +320,15 @@ int build_storage(rf_dit* h) {
     b.to_out = new_lin(h, ar, p + "attn.to_out.0", D, D);
     new_lora(h, ar, p + "attn.to_out.0", b.l_out, D, D);
     b.to_add_out = new_lin(h, ar, p + "attn.to_add_out", D, D);
+    new_always_lora(h, p + "attn.to_add_out", b.l_add_out, D, D);
     b.ff1 = new_lin(h, ar, p + "ff.net.0.proj", 4 * D, D);
+    new_always_lora(h, p + "ff.net.0.proj", b.l_ff1, 4 * D, D);
     b.ff2 = new_lin(h, ar, p + "ff.net.2", D, 4 * D);
     new_lora(h, ar, p + "ff.net.2", b.l_ff2, D, 4 * D);
     b.ffc1 = new_lin(h, ar, p + "ff_context.net.0.proj", 4 * D, D);
     b.ffc2 = new_lin(h, ar, p + "ff_context.net.2", D, 4 * D);
+    new_always_lora(h, p + "ff_context.net.0.proj", b.l_ffc1, 4 * D, D);
+    new_always_lora(h, p + "ff_context.net.2", b.l_ffc2, D, 4 * D);
   }
   h->sgl.resize(c.num_single_layers);
   const int64_t so = static_cast<int64_t>(c.num_layers) * 12 * D;
@@ -285,6 +363,7 @@ int build_storage(rf_dit* h) {
   }
   const int64_t oo = so + static_cast<int64_t>(c.num_single_layers) * 3 * D;
   reg_lin(h, "norm_out.linear", h->modW + oo * D, h->modB + oo, 2 * D, D);
+  new_always_lora(h, "norm_out.linear", h->l_norm_out, 2 * D, D);
   return ar.fail;
 }
 
@@ -303,18 +382,28 @@ inline int64_t mod_out(const rf_dit* h, int which) {
 }
 enum { SHIFT_MSA = 0, SCALE_MSA = 1, GATE_MSA = 2, SHIFT_MLP = 3, SCALE_MLP = 4, GATE_MLP = 5 };
 
-#define RF_TRY(expr)            \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != 0) return _rc;   \
-  } while (0)
+// The low-rank term of a Linear that runs as a GEMV (embedders, adaLN), for `batch` vectors:
+// y[b] = bf16(y[b] + bf16(bf16(bf16(act(x_b) A^T) B^T) * scaling)) (peft), act = silu when act = 1, as in the GEMV of
+// the Linear itself.  Two batched GEMVs and one strided add; tvec [batch, lora_pad], lvec [batch, t.out] scratch.
+int add_vec_lora(rf_dit* h, const LoraT& t, const bf16* x, int ldx, int batch, int act, bf16* y, int64_t ldy,
+                 bf16* tvec, bf16* lvec, cudaStream_t s) {
+  if (!lora_on(h, t)) return 0;
+  const int lpad = h->lora_pad;
+  RF_TRY(rf::gemv_launch(x, ldx, batch, t.A, nullptr, tvec, lpad, lpad, t.in, act, s));
+  RF_TRY(rf::gemv_launch(tvec, lpad, batch, t.B, nullptr, lvec, t.out, t.out, lpad, 0, s));
+  return rf::add_rows_launch(y, ldy, lvec, t.out, batch, t.out, lora_eff(h, t), s);
+}
 
-// y = linear_2(silu(linear_1(x)))  (TimestepEmbedding / PixArtAlphaTextProjection)
-int mlp2(rf_dit* h, const bf16* x, int in_dim, const Lin& l1, const Lin& l2, bf16* tmp, bf16* out,
-         cudaStream_t s) {
-  RF_TRY(rf::gemv_launch(x, in_dim, 1, l1.w, l1.b, tmp, h->D, h->D, in_dim, 0, s));
-  RF_TRY(rf::gemv_launch(tmp, h->D, 1, l2.w, l2.b, out, h->D, h->D, h->D, 1, s));
-  return 0;
+// y = linear_2(silu(linear_1(x)))  (TimestepEmbedding / PixArtAlphaTextProjection) for `batch` vectors, each Linear
+// with its LoRA term (always targets): linear_2's sees the same bf16(silu(.)) input as its GEMV.
+// tvec [batch, lora_pad], lvec [batch, D] scratch.
+int mlp2(rf_dit* h, const bf16* x, int in_dim, int batch, const Lin& l1, const LoraT& lt1, const Lin& l2,
+         const LoraT& lt2, bf16* tmp, bf16* out, bf16* tvec, bf16* lvec, cudaStream_t s) {
+  const int D = h->D;
+  RF_TRY(rf::gemv_launch(x, in_dim, batch, l1.w, l1.b, tmp, D, D, in_dim, 0, s));
+  RF_TRY(add_vec_lora(h, lt1, x, in_dim, batch, 0, tmp, D, tvec, lvec, s));
+  RF_TRY(rf::gemv_launch(tmp, D, batch, l2.w, l2.b, out, D, D, D, 1, s));
+  return add_vec_lora(h, lt2, tmp, D, batch, 1, out, D, tvec, lvec, s);
 }
 
 // temb = time(t) + guidance(g) + text(pooled)   (CombinedTimestepGuidanceTextProjEmbeddings)
@@ -323,12 +412,13 @@ int compute_temb(rf_dit* h, const bf16* t, const int* step, const bf16* guid, co
   const int D = h->D;
   bf16* e = h->emb_tmp;  // [256 | 256 | D tmp | D a | D b | D c]
   bf16 *tp = e, *gp = e + 256, *tmp = e + 512, *a = tmp + D, *b = a + D, *c = b + D;
+  bf16 *tvec = h->LT, *lvec = h->LT + 256;  // embedder LoRA scratch: [lora_pad] | [D] (LT holds >= 8D)
   RF_TRY(rf::timestep_embed_launch(t, step, 1, 1000.0f, tp, 1, s));
-  RF_TRY(mlp2(h, tp, 256, h->t1, h->t2, tmp, a, s));
-  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, h->p1, h->p2, tmp, c, s));
+  RF_TRY(mlp2(h, tp, 256, 1, h->t1, h->l_t1, h->t2, h->l_t2, tmp, a, tvec, lvec, s));
+  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, 1, h->p1, h->l_p1, h->p2, h->l_p2, tmp, c, tvec, lvec, s));
   if (h->cfg.guidance_embeds) {
     RF_TRY(rf::timestep_embed_launch(guid, nullptr, 1, 1000.0f, gp, 1, s));
-    RF_TRY(mlp2(h, gp, 256, h->g1, h->g2, tmp, b, s));
+    RF_TRY(mlp2(h, gp, 256, 1, h->g1, h->l_g1, h->g2, h->l_g2, tmp, b, tvec, lvec, s));
     RF_TRY(rf::add3_launch(a, b, c, out, D, s));
   } else {
     RF_TRY(rf::add2_launch(a, c, out, D, s));
@@ -362,22 +452,26 @@ int lora_term(rf_dit* h, const LoraT* const* ls, int n, const bf16* A_all, const
   return rf::gemm_launch(scaled ? rf::EPI_SCALE : rf::EPI_BIAS, ls[0]->out, lpad, n, g, s);
 }
 
-// The low-rank term of the adaLN Linears (norm1.linear of the double blocks, norm.linear of the single blocks)
-// added to their sections of `batch` modulation rows: mod[b * ld_mod + section] += bf16(bf16(silu(emb_b) A^T) B^T)
-// (peft: bf16(y + L)).  M = batch is tiny: two batched GEMVs and one strided add per target.
-// The scaling is applied in the add: mod += bf16(L * scaling).
+// The low-rank term of the adaLN Linears added to their sections of `batch` modulation rows:
+// mod[b * ld_mod + section] += bf16(bf16(bf16(silu(emb_b) A^T) B^T) * scaling) (peft: bf16(y + L)).  `gated`: the
+// targets enable_lora names (norm1.linear of the double blocks, norm.linear of the single blocks); `always`: the
+// text-stream norm1_context.linear and norm_out.linear, which no enable_lora names.
+// M = batch is tiny: two batched GEMVs and one strided add per target.
 // tvec: [batch, lora_pad], lvec: [batch, 6D] scratch.
-int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bf16* mod, int64_t ld_mod, bf16* tvec, bf16* lvec,
-                 cudaStream_t s) {
-  const int D = h->D, lpad = h->lora_pad;
-  auto one = [&](const LoraT& t, int64_t off) -> int {
-    if (!lora_on(h, t)) return 0;
-    RF_TRY(rf::gemv_launch(emb, D, batch, t.A, nullptr, tvec, lpad, lpad, D, 1, s));
-    RF_TRY(rf::gemv_launch(tvec, lpad, batch, t.B, nullptr, lvec, t.out, t.out, lpad, 0, s));
-    return rf::add_rows_launch(mod + off, ld_mod, lvec, t.out, batch, t.out, lora_eff(h, t), s);
+int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bool gated, bool always, bf16* mod, int64_t ld_mod,
+                 bf16* tvec, bf16* lvec, cudaStream_t s) {
+  const int D = h->D;
+  auto one = [&](const LoraT& t, int64_t off) {
+    return add_vec_lora(h, t, emb, D, batch, 1, mod + off, ld_mod, tvec, lvec, s);
   };
-  for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1, mod_double(h, i, 0, 0)));
-  for (int i = 0; i < h->cfg.num_single_layers; ++i) RF_TRY(one(h->sgl[i].l_norm, mod_single(h, i, 0)));
+  if (gated) {
+    for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1, mod_double(h, i, 0, 0)));
+    for (int i = 0; i < h->cfg.num_single_layers; ++i) RF_TRY(one(h->sgl[i].l_norm, mod_single(h, i, 0)));
+  }
+  if (always && h->any_always) {
+    for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1c, mod_double(h, i, 1, 0)));
+    RF_TRY(one(h->l_norm_out, mod_out(h, 0)));
+  }
   return 0;
 }
 
@@ -389,8 +483,9 @@ int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
   RF_TRY(rf::gemv_launch(h->ctemb, D, 1, h->modW, h->modB, h->MODC, static_cast<int>(h->n_mod),
                          static_cast<int>(h->n_mod), D, 1, s));
   if (!h->any_lora) return 0;
-  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb); tvec [1, lora_pad <= 256] at the front of LT
-  return add_mod_lora(h, h->ctemb, 1, h->MODC, h->n_mod, h->LT, h->LT + 256, s);
+  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb); tvec [1, lora_pad <= 256] at the front of LT.  (The
+  // condition rows read no norm1_context / norm_out section of MODC.)
+  return add_mod_lora(h, h->ctemb, 1, true, false, h->MODC, h->n_mod, h->LT, h->LT + 256, s);
 }
 
 // fuse_lora mode: merged weights for the condition-token groups (allocated on first use)
@@ -410,15 +505,38 @@ int merge_one(rf_dit* h, const LoraT& t, const bf16* W, bf16** Wm, int rows_off,
   }
   return rf::lora_merge_launch(W + off, t.A, t.B, *Wm + off, t.out, t.in, h->lora_pad, lora_eff(h, t), s);
 }
+// an always target (or pack) has a merged copy only once one of its targets is set; until then its groups read the
+// base weight (any_set), so a handle without such adapters allocates nothing here
+bool any_set(const LoraT* const* ls, int n) {
+  for (int k = 0; k < n; ++k)
+    if (ls[k]->set) return true;
+  return false;
+}
+int merge_always(rf_dit* h, const LoraT* const* ls, int n, const bf16* W, bf16** Wm, cudaStream_t s) {
+  if (!any_set(ls, n)) return 0;
+  for (int k = 0; k < n; ++k) RF_TRY(merge_one(h, *ls[k], W, Wm, k * ls[k]->out, n * ls[k]->out, s));
+  return 0;
+}
 int merge_all(rf_dit* h, cudaStream_t s) {
   const int D = h->D;
   RF_TRY(merge_one(h, h->l_x_emb, h->x_emb.w, &h->x_emb_m, 0, D, s));
+  const LoraT* lctx = &h->l_ctx;
+  const LoraT* lpo = &h->l_proj_out;
+  RF_TRY(merge_always(h, &lctx, 1, h->ctx_emb.w, &h->ctx_emb_m, s));
+  RF_TRY(merge_always(h, &lpo, 1, h->proj_out.w, &h->proj_out_m, s));
   for (auto& b : h->dbl) {
     RF_TRY(merge_one(h, b.l_q, b.qkv.w, &b.qkv_m, 0, 3 * D, s));
     RF_TRY(merge_one(h, b.l_k, b.qkv.w, &b.qkv_m, D, 3 * D, s));
     RF_TRY(merge_one(h, b.l_v, b.qkv.w, &b.qkv_m, 2 * D, 3 * D, s));
     RF_TRY(merge_one(h, b.l_out, b.to_out.w, &b.to_out_m, 0, D, s));
     RF_TRY(merge_one(h, b.l_ff2, b.ff2.w, &b.ff2_m, 0, D, s));
+    const LoraT* la[3] = {&b.l_aq, &b.l_ak, &b.l_av};
+    const LoraT *lao = &b.l_add_out, *lf1 = &b.l_ff1, *lc1 = &b.l_ffc1, *lc2 = &b.l_ffc2;
+    RF_TRY(merge_always(h, la, 3, b.add_qkv.w, &b.add_qkv_m, s));
+    RF_TRY(merge_always(h, &lao, 1, b.to_add_out.w, &b.to_add_out_m, s));
+    RF_TRY(merge_always(h, &lf1, 1, b.ff1.w, &b.ff1_m, s));
+    RF_TRY(merge_always(h, &lc1, 1, b.ffc1.w, &b.ffc1_m, s));
+    RF_TRY(merge_always(h, &lc2, 1, b.ffc2.w, &b.ffc2_m, s));
   }
   for (auto& b : h->sgl) {
     RF_TRY(merge_one(h, b.l_q, b.qkv.w, &b.qkv_m, 0, 3 * D, s));
@@ -447,13 +565,15 @@ int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16*
   bf16* temb = a + static_cast<int64_t>(n_steps) * D;
   bf16* gp = temb + static_cast<int64_t>(n_steps) * D;
   bf16 *tmp1 = gp + 256, *b = tmp1 + D, *c = b + D;
+  bf16* tvec = c + D;                                               // [n, lora_pad]
+  bf16* lvec = tvec + static_cast<int64_t>(n_steps) * h->lora_pad;  // [n, 6D]
   RF_TRY(rf::timestep_embed_launch(tsteps, nullptr, 1, 1000.0f, tp, n_steps, s));
-  RF_TRY(rf::gemv_launch(tp, 256, n_steps, h->t1.w, h->t1.b, tmp, D, D, 256, 0, s));
-  RF_TRY(rf::gemv_launch(tmp, D, n_steps, h->t2.w, h->t2.b, a, D, D, D, 1, s));
-  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, h->p1, h->p2, tmp1, c, s));
+  // the timestep embedder and its LoRA terms batched over every step, like compute_temb per vector
+  RF_TRY(mlp2(h, tp, 256, n_steps, h->t1, h->l_t1, h->t2, h->l_t2, tmp, a, tvec, lvec, s));
+  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, 1, h->p1, h->l_p1, h->p2, h->l_p2, tmp1, c, tvec, lvec, s));
   if (h->cfg.guidance_embeds) {
     RF_TRY(rf::timestep_embed_launch(guid, nullptr, 1, 1000.0f, gp, 1, s));
-    RF_TRY(mlp2(h, gp, 256, h->g1, h->g2, tmp1, b, s));
+    RF_TRY(mlp2(h, gp, 256, 1, h->g1, h->l_g1, h->g2, h->l_g2, tmp1, b, tvec, lvec, s));
   }
   for (int i = 0; i < n_steps; ++i) {
     bf16* ai = a + static_cast<int64_t>(i) * D;
@@ -463,13 +583,11 @@ int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16*
   }
   RF_TRY(rf::gemv_launch(temb, D, n_steps, h->modW, h->modB, h->s_mod_all, static_cast<int>(h->n_mod),
                          static_cast<int>(h->n_mod), D, 1, s));
-  // latent_lora: the adaLN LoRA of the image stream (double blocks) / of the txt+img rows (single blocks) acts on
-  // silu(temb_i), which every step knows before the loop: its term joins the table here too
-  if ((h->flags & 1) && h->any_lora) {
-    bf16* tvec = c + D;                                               // [n, lora_pad]
-    bf16* lvec = tvec + static_cast<int64_t>(n_steps) * h->lora_pad;  // [n, 6D]
-    RF_TRY(add_mod_lora(h, temb, n_steps, h->s_mod_all, h->n_mod, tvec, lvec, s));
-  }
+  // the adaLN LoRA terms act on silu(temb_i), which every step knows before the loop: they join the table here too
+  // (latent_lora: the image stream of the double blocks / the txt+img rows of the single blocks; always:
+  // norm1_context and norm_out)
+  if (h->any_lora) RF_TRY(add_mod_lora(h, temb, n_steps, (h->flags & 1) != 0, true, h->s_mod_all, h->n_mod, tvec,
+                                       lvec, s));
   return 0;
 }
 
@@ -519,6 +637,14 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   memset(g, 0, sizeof(g));
   g[0].A = txt; g[0].lda = h->cfg.joint_attention_dim; g[0].M = h->n_txt; g[0].W = h->ctx_emb.w;
   g[0].bias = h->ctx_emb.b; g[0].out = rowp(X, D, 0); g[0].ldo = D;
+  // context_embedder (always target; EPI_BIAS, K = 4096): the unfused term, like x_embedder's
+  const LoraT* lctx = &h->l_ctx;
+  if (h->use_merged) {
+    if (lctx->set) g[0].W = h->ctx_emb_m;
+  } else if (lora_on(h, *lctx)) {
+    RF_TRY(lora_term(h, &lctx, 1, lctx->A, txt, g[0].lda, g[0].M, nullptr, 0, h->LL, D, s));
+    g[0].addend = h->LL; g[0].ldadd = D;
+  }
   RF_TRY(rf::gemm_launch(rf::EPI_BIAS, D, h->cfg.joint_attention_dim, 1, g, s));
 
   // ---- temb and every modulation vector of the step (transformer.py:95-107 + all adaLN linears)
@@ -528,7 +654,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     RF_TRY(compute_temb(h, tstep, step_idx, guid, pooled, h->temb, s));
     RF_TRY(rf::gemv_launch(h->temb, D, 1, h->modW, h->modB, h->MOD, static_cast<int>(h->n_mod),
                            static_cast<int>(h->n_mod), D, 1, s));
-    if (ll && h->any_lora) RF_TRY(add_mod_lora(h, h->temb, 1, h->MOD, h->n_mod, h->LT, h->LT + 256, s));
+    if (h->any_lora) RF_TRY(add_mod_lora(h, h->temb, 1, ll, true, h->MOD, h->n_mod, h->LT, h->LT + 256, s));
   }
   const bf16* MOD = h->MOD;
   const bf16* MODC = h->MODC;
@@ -537,57 +663,94 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     return rf::ln_modulate_launch(rowp(X, D, sr.row0), D, rowp(XN, D, sr.row0), D, sr.rows, D, scale,
                                   shift, sr.rows, 0, s);
   };
-  // The groups of a projection launch that carry the LoRA in exact mode, in row order: the image (double blocks) or
-  // txt + img (single blocks) group under latent_lora, then the condition group.  Their rows are contiguous in the
-  // joint buffers ([n_txt, N) resp. [0, N)), so one down-projection over that range serves all of them; `row` is
-  // each group's first row inside the range, i.e. its row in LT / LL.
+  // The groups of a projection launch that carry the LoRA in exact mode, in row order, each with its target(s) `ls`
+  // and stacked factors A_all / B_all: in the double blocks the text group (its own add_* / to_add_out / ff_context
+  // targets, always on), the image group (under latent_lora; always for ff.net.0.proj), the condition group; in the
+  // single blocks the txt + img group under latent_lora, then the condition group.  `row` is each group's row in
+  // LT / LL: groups are stacked there in this order.
+  struct LoraGrp {
+    int idx, row;
+    const LoraT* const* ls;
+    const bf16 *A_all, *B_all;
+  };
   struct LoraGroups {
     int n = 0, rows = 0;
-    int idx[2] = {0, 0};
-    int row[2] = {0, 0};
-    void add(int i, int m) { idx[n] = i; row[n] = rows; rows += m; ++n; }
+    LoraGrp e[3];
+    void add(int i, int m, const LoraT* const* ls, const bf16* A_all, const bf16* B_all) {
+      e[n] = LoraGrp{i, rows, ls, A_all, B_all};
+      rows += m;
+      ++n;
+    }
   };
-  auto lora_groups = [&](bool target_set, int main_idx, int main_rows, int cond_idx) {
+  // on: the target(s) of the image (double) / main (single) and condition groups add a term; main_always: the image
+  // group carries it whatever latent_lora says (ff.net.0.proj)
+  auto lora_groups = [&](bool on, int main_idx, int main_rows, int cond_idx, const LoraT* const* ls,
+                         const bf16* A_all, const bf16* B_all, bool main_always = false) {
     LoraGroups lg;
-    if (!target_set || h->use_merged) return lg;
-    if (ll) lg.add(main_idx, main_rows);
-    if (use_cond) lg.add(cond_idx, h->n_cond);
+    if (!on || h->use_merged) return lg;
+    if (ll || main_always) lg.add(main_idx, main_rows, ls, A_all, B_all);
+    if (use_cond) lg.add(cond_idx, h->n_cond, ls, A_all, B_all);
+    return lg;
+  };
+  // the double blocks: the text group (always targets) first, then the image / condition groups
+  auto lora_groups_dbl = [&](bool txt_on, const LoraT* const* txt_ls, const bf16* txt_A, const bf16* txt_B,
+                             bool on, const LoraT* const* ls, const bf16* A_all, const bf16* B_all,
+                             bool main_always = false) {
+    LoraGroups lg;
+    if (h->use_merged) return lg;
+    if (txt_on) lg.add(1, h->n_txt, txt_ls, txt_A, txt_B);
+    if (on && (ll || main_always)) lg.add(0, h->n_img, ls, A_all, B_all);
+    if (on && use_cond) lg.add(2, h->n_cond, ls, A_all, B_all);
     return lg;
   };
   // merged mode (fuse_lora): the same groups read the merged weights W + B A instead
-  auto merged_w = [&](rf::GemmGroupArgs* gr, int main_idx, int cond_idx, const bf16* Wm) {
+  auto merged_w = [&](rf::GemmGroupArgs* gr, int main_idx, int cond_idx, const bf16* Wm, bool main_always = false) {
     if (!h->use_merged) return;
-    if (ll) gr[main_idx].W = Wm;
+    if (ll || main_always) gr[main_idx].W = Wm;
     if (use_cond) gr[cond_idx].W = Wm;
   };
-  // A grouped GEMM in which the groups `lg` carry the LoRA of `ls` (one target, or the three stacked q|k|v
-  // targets; A_all / B_all their stacked factors).  Fast path: T = bf16(x A^T) for all LoRA'd rows (one skinny
-  // GEMM), then ONE grouped launch of all streams in which the eligible groups' tiles carry the low-rank k-block
-  // (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Groups too small for it (gemm_lora_eligible) keep the
-  // unfused path: L materialised in their rows of LL and added in the epilogue (`addend`); they reuse T when it
-  // exists.  (t_pre != nullptr: T was already produced by an earlier launch, [rows, ld_t] with this target's
-  // columns at t_pre.)
-  auto gemm_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const LoraGroups& lg,
-                       const LoraT* const* ls, int nls, const bf16* A_all, const bf16* B_all, int ldl,
-                       const bf16* t_pre = nullptr, int ld_t = 0) -> int {
-    bool fused[2] = {false, false}, any_fused = false;
-    for (int j = 0; j < lg.n; ++j) any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, gr[lg.idx[j]]));
+  // A grouped GEMM in which the groups `lg` carry their LoRA (nls = 1 target each, or 3 stacked q|k|v targets).
+  // Fast path: T = bf16(x A^T) for all LoRA'd rows in one skinny grouped GEMM (one group per run of rows that are
+  // contiguous in the A operand and share their A factors), then ONE grouped launch of all streams in which the
+  // eligible groups' tiles carry the low-rank k-block (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Groups
+  // too small for it (gemm_lora_eligible) keep the unfused path: L materialised in their rows of LL and added in the
+  // epilogue (`addend`); they reuse T when it exists.  (t_pre != nullptr: T was already produced by an earlier
+  // launch, [rows, ld_t] with this target's columns at t_pre.)
+  auto gemm_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const LoraGroups& lg, int nls,
+                       int ldl, const bf16* t_pre = nullptr, int ld_t = 0) -> int {
+    bool fused[3] = {false, false, false}, any_fused = false;
+    for (int j = 0; j < lg.n; ++j) any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, gr[lg.e[j].idx]));
     if (any_fused && t_pre == nullptr) {
-      const rf::GemmGroupArgs& g0 = gr[lg.idx[0]];
-      RF_TRY(rf::lora_down_launch(g0.A, g0.lda, lg.rows, K, A_all, nls * lpad, h->LT, nls * lpad, s));
-      t_pre = h->LT;
       ld_t = nls * lpad;
+      rf::GemmGroupArgs dg[3];
+      memset(dg, 0, sizeof(dg));
+      int nd = 0;
+      for (int j = 0; j < lg.n; ++j) {
+        const rf::GemmGroupArgs& gc = gr[lg.e[j].idx];
+        rf::GemmGroupArgs* last = nd ? &dg[nd - 1] : nullptr;
+        if (last && last->W == lg.e[j].A_all && last->lda == gc.lda &&
+            gc.A == last->A + static_cast<int64_t>(last->M) * last->lda) {
+          last->M += gc.M;
+          continue;
+        }
+        dg[nd].A = gc.A; dg[nd].lda = gc.lda; dg[nd].M = gc.M; dg[nd].W = lg.e[j].A_all;
+        dg[nd].out = h->LT + static_cast<int64_t>(lg.e[j].row) * ld_t; dg[nd].ldo = ld_t;
+        ++nd;
+      }
+      RF_TRY(rf::lora_down_launch(K, ld_t, nd, dg, s));
+      t_pre = h->LT;
     }
     for (int j = 0; j < lg.n; ++j) {
-      rf::GemmGroupArgs& gc = gr[lg.idx[j]];
-      const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(lg.row[j]) * ld_t : nullptr;
+      const LoraGrp& e = lg.e[j];
+      rf::GemmGroupArgs& gc = gr[e.idx];
+      const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(e.row) * ld_t : nullptr;
       if (fused[j]) {
-        gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = B_all; gc.lora_sec_cols = nls > 1 ? ls[0]->out : 0;
+        gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = e.B_all; gc.lora_sec_cols = nls > 1 ? e.ls[0]->out : 0;
         gc.lora_pad = lpad;
-        for (int k = 0; k < nls; ++k) gc.lora_scale[k] = lora_eff(h, *ls[k]);
+        for (int k = 0; k < nls; ++k) gc.lora_scale[k] = lora_eff(h, *e.ls[k]);
       } else {
-        bf16* L = rowp(h->LL, ldl, lg.row[j]);
-        RF_TRY(lora_term(h, ls, nls, A_all, gc.A, gc.lda, gc.M, t_rows, ld_t, L, ldl, s));
+        bf16* L = rowp(h->LL, ldl, e.row);
+        RF_TRY(lora_term(h, e.ls, nls, e.A_all, gc.A, gc.lda, gc.M, t_rows, ld_t, L, ldl, s));
         gc.addend = L; gc.ldadd = ldl;
       }
     }
@@ -637,8 +800,13 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 2, b.qkv_m);
     const LoraT* dqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_img.rows, 2);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, dqkv, 3, b.qkvA, b.qkvB, D3));
+    const LoraT* dadd[3] = {&b.l_aq, &b.l_ak, &b.l_av};
+    if (h->use_merged && any_set(dadd, 3)) g[1].W = b.add_qkv_m;
+    LoraGroups lg = lora_groups_dbl(lora_on(h, b.l_aq) || lora_on(h, b.l_ak) || lora_on(h, b.l_av), dadd,
+                                    b.add_qkvA, b.add_qkvB,
+                                    lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), dqkv, b.qkvA,
+                                    b.qkvB);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, 3, D3));
     else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // joint attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
@@ -660,8 +828,11 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 2, b.to_out_m);
     const LoraT* dout = &b.l_out;
-    lg = lora_groups(lora_on(h, b.l_out), 0, S_img.rows, 2);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D, ng, g, lg, &dout, 1, b.l_out.A, b.l_out.B, D));
+    const LoraT* dadd_out = &b.l_add_out;
+    if (h->use_merged && b.l_add_out.set) g[1].W = b.to_add_out_m;
+    lg = lora_groups_dbl(lora_on(h, b.l_add_out), &dadd_out, b.l_add_out.A, b.l_add_out.B, lora_on(h, b.l_out),
+                         &dout, b.l_out.A, b.l_out.B);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D, ng, g, lg, 1, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D, ng, g, s));
     // norm2 + modulate
     RF_TRY(ln3(mt + SCALE_MLP * D, mt + SHIFT_MLP * D, mi + SCALE_MLP * D, mi + SHIFT_MLP * D,
@@ -680,7 +851,15 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
       g[2].out = rowp(ACT, D5, S_cond.row0) + D;
       ng = 3;
     }
-    RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
+    // ff.net.0.proj is inside no enable_lora (block.py:250 names ff.net[2] only): its image rows always carry it
+    if (b.l_ff1.set) merged_w(g, 0, 2, b.ff1_m, true);
+    if (h->use_merged && b.l_ffc1.set) g[1].W = b.ffc1_m;
+    const LoraT* dff1 = &b.l_ff1;
+    const LoraT* dffc1 = &b.l_ffc1;
+    lg = lora_groups_dbl(lora_on(h, b.l_ffc1), &dffc1, b.l_ffc1.A, b.l_ffc1.B, lora_on(h, b.l_ff1), &dff1,
+                         b.l_ff1.A, b.l_ff1.B, true);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, 1, D4));
+    else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
     // MLP out + gate + residual
     memset(g, 0, sizeof(g));
     g[0].A = rowp(ACT, D5, S_img.row0) + D; g[0].lda = D5; g[0].M = S_img.rows; g[0].W = b.ff2.w;
@@ -697,9 +876,12 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
       ng = 3;
     }
     merged_w(g, 0, 2, b.ff2_m);
+    if (h->use_merged && b.l_ffc2.set) g[1].W = b.ffc2_m;
     const LoraT* dff2 = &b.l_ff2;
-    lg = lora_groups(lora_on(h, b.l_ff2), 0, S_img.rows, 2);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D4, ng, g, lg, &dff2, 1, b.l_ff2.A, b.l_ff2.B, D));
+    const LoraT* dffc2 = &b.l_ffc2;
+    lg = lora_groups_dbl(lora_on(h, b.l_ffc2), &dffc2, b.l_ffc2.A, b.l_ffc2.B, lora_on(h, b.l_ff2), &dff2,
+                         b.l_ff2.A, b.l_ff2.B);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D4, ng, g, lg, 1, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D4, ng, g, s));
   }
 
@@ -726,19 +908,19 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.qkv_m);
     const LoraT* sqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_main.rows, 1);
+    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_main.rows, 1,
+                                sqkv, b.qkvA, b.qkvB);
     // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp of all LoRA'd rows in one launch (both GEMMs read the
     // same XN rows; the q|k|v and the MLP-in launches have the same groups)
     bool t4 = lg.n > 0 && lora_on(h, b.l_mlp);
     if (t4) {
       bool any_fused = false;
-      for (int j = 0; j < lg.n; ++j) any_fused |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[lg.idx[j]]);
+      for (int j = 0; j < lg.n; ++j) any_fused |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[lg.e[j].idx]);
       t4 = any_fused;
     }
     if (t4)
-      RF_TRY(rf::lora_down_launch(g[lg.idx[0]].A, D, lg.rows, D, b.qkvA, 4 * lpad, h->LT, 4 * lpad, s));
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, sqkv, 3, b.qkvA, b.qkvB, D3, t4 ? h->LT : nullptr,
-                               4 * lpad));
+      RF_TRY(rf::lora_down_launch(g[lg.e[0].idx].A, D, lg.rows, D, b.qkvA, 4 * lpad, h->LT, 4 * lpad, s));
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, 3, D3, t4 ? h->LT : nullptr, 4 * lpad));
     else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
     // proj_mlp + GELU -> ACT[:, D:5D]
     memset(g, 0, sizeof(g));
@@ -753,9 +935,8 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.mlp_m);
     const LoraT* smlp = &b.l_mlp;
-    lg = lora_groups(lora_on(h, b.l_mlp), 0, S_main.rows, 1);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, &smlp, 1, b.l_mlp.A, b.l_mlp.B, D4,
-                               t4 ? h->LT + 3 * lpad : nullptr, 4 * lpad));
+    lg = lora_groups(lora_on(h, b.l_mlp), 0, S_main.rows, 1, &smlp, b.l_mlp.A, b.l_mlp.B);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, 1, D4, t4 ? h->LT + 3 * lpad : nullptr, 4 * lpad));
     else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
     // attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
@@ -773,8 +954,8 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     }
     merged_w(g, 0, 1, b.out_m);
     const LoraT* sout = &b.l_out;
-    lg = lora_groups(lora_on(h, b.l_out), 0, S_main.rows, 1);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D5, ng, g, lg, &sout, 1, b.l_out.A, b.l_out.B, D));
+    lg = lora_groups(lora_on(h, b.l_out), 0, S_main.rows, 1, &sout, b.l_out.A, b.l_out.B);
+    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D5, ng, g, lg, 1, D));
     else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D5, ng, g, s));
   }
 
@@ -784,13 +965,39 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   memset(g, 0, sizeof(g));
   g[0].A = rowp(XN, D, S_img.row0); g[0].lda = D; g[0].M = S_img.rows; g[0].W = h->proj_out.w;
   g[0].bias = h->proj_out.b; g[0].out = out; g[0].ldo = h->cfg.in_channels;
+  // proj_out (always target; N = 64): the unfused term
+  const LoraT* lpo = &h->l_proj_out;
+  if (h->use_merged) {
+    if (lpo->set) g[0].W = h->proj_out_m;
+  } else if (lora_on(h, *lpo)) {
+    RF_TRY(lora_term(h, &lpo, 1, lpo->A, g[0].A, g[0].lda, g[0].M, nullptr, 0, h->LL, h->cfg.in_channels, s));
+    g[0].addend = h->LL; g[0].ldadd = h->cfg.in_channels;
+  }
   RF_TRY(rf::gemm_launch(rf::EPI_BIAS, h->cfg.in_channels, D, 1, g, s));
   return 0;
 }
 
-// fuse_lora mode applies when some group carries a LoRA: the condition stream, or the image under latent_lora
+// fuse_lora mode applies when some group carries a LoRA: the condition stream, the image under latent_lora, or the
+// rows of an always target
 bool wants_merged(const rf_dit* h, int n_cond) {
-  return (h->flags & 8) != 0 && h->any_lora && (n_cond > 0 || (h->flags & 1) != 0);
+  return (h->flags & 8) != 0 && h->any_lora && (n_cond > 0 || (h->flags & 1) != 0 || h->any_always);
+}
+
+// rows that can carry a LoRA term (LT / LL): the condition stream, plus txt + img under latent_lora (the single
+// blocks LoRA every main row) or with an always target set (text stream, image rows of ff.net.0.proj / proj_out)
+int lora_rows_needed(const rf_dit* h, int flags, int N, int n_cond) {
+  return std::max(((flags & 1) || h->any_always) ? N : n_cond, 1);
+}
+// LT [rows, 4 lora_pad] and LL [rows, 4D], each at least 8D (the adaLN / embedder LoRA scratch)
+int alloc_lora_ws(rf_dit* h, int rows) {
+  const size_t r = static_cast<size_t>(rows), least = static_cast<size_t>(8 * h->D) * 2;
+  void* p = nullptr;
+  RF_TRY(dev_alloc(h, &p, std::max(r * 4 * h->lora_pad * 2, least), true));
+  h->LT = static_cast<bf16*>(p);
+  RF_TRY(dev_alloc(h, &p, std::max(r * 4 * h->D * 2, least), true));
+  h->LL = static_cast<bf16*>(p);
+  h->lora_rows = rows;
+  return 0;
 }
 // the merged copies hold W + (B A) * scaling for the current weights, adapters and call scale
 bool merged_current(const rf_dit* h) { return h->lora_merged && h->merged_call_scale == h->call_scale; }
@@ -998,7 +1205,8 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
   }
   auto it = h->lora_slots.find(module);
   if (it == h->lora_slots.end()) {
-    rf::set_error(std::string("rf_dit_set_lora: not a LoRA target (or lora_rank == 0): ") + module);
+    rf::set_error(std::string("rf_dit_set_lora: not a Linear of FluxTransformer2DModel (or lora_rank == 0): ") +
+                  module);
     return -4;
   }
   if (r <= 0 || r > h->cfg.lora_rank) {
@@ -1018,6 +1226,7 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
                   " out=" + std::to_string(out_features));
     return -4;
   }
+  RF_TRY(lora_storage(h, t));
   RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(lpad) * t.in * 2));
   RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * lpad * 2));
   RF_CHECK_CUDA(cudaMemcpy(t.A, A, static_cast<size_t>(r) * t.in * 2, cudaMemcpyDeviceToDevice));
@@ -1026,8 +1235,32 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
   t.set = true;
   t.scale = scale;
   h->any_lora = true;
+  h->any_always |= t.always;
   h->lora_merged = false;
   drop_graph(h);  // the captured step may predate this adapter (different launch list)
+  return 0;
+}
+
+int rf_dit_clear_lora(rf_dit* h) {
+  if (!h) {
+    rf::set_error("rf_dit_clear_lora: null handle");
+    return -1;
+  }
+  const int lpad = h->lora_pad;
+  for (auto& kv : h->lora_slots) {
+    LoraT& t = *kv.second;
+    // zeroed: an unset member of a stacked q|k|v pack still runs in its pack's GEMMs and must add exactly nothing
+    if (t.set) {
+      RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(lpad) * t.in * 2));
+      RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * lpad * 2));
+    }
+    t.set = false;
+    t.scale = 1.0;
+  }
+  h->any_lora = false;
+  h->any_always = false;
+  h->lora_merged = false;
+  drop_graph(h);
   return 0;
 }
 
@@ -1088,9 +1321,7 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (flags & 4) mode = 2;  // union_cond_attn == False wins only if no c_factor...
     if ((flags & 4) && condition_scale != 1.0f) mode = 1;  // c_factor mask overrides (block.py:115)
   }
-  // rows that can carry a LoRA term (LT / LL): the condition stream, plus txt + img under latent_lora (the single
-  // blocks LoRA every main row; the double blocks only the image rows)
-  const int lora_rows = std::max((flags & 1) ? N : n_cond, 1);
+  const int lora_rows = lora_rows_needed(h, flags, N, n_cond);
   const bool same = h->prepared && h->batch == batch && h->n_txt == n_txt && h->n_img == n_img &&
                     h->n_cond == n_cond && h->lora_rows >= lora_rows;
   if (same) drop_graph(h); else free_geometry(h);
@@ -1122,10 +1353,7 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (!(p = A(static_cast<size_t>(N) * 5 * D * 2))) return -2; h->ACT = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MOD = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MODC = static_cast<bf16*>(p);
-    h->lora_rows = lora_rows;
-    const size_t lrows = static_cast<size_t>(lora_rows);
-    if (!(p = A(std::max(lrows * 4 * h->lora_pad * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LT = static_cast<bf16*>(p);
-    if (!(p = A(std::max(lrows * 4 * D * 2, static_cast<size_t>(8 * D) * 2)))) return -2; h->LL = static_cast<bf16*>(p);
+    RF_TRY(alloc_lora_ws(h, lora_rows));
     if (!(p = A(static_cast<size_t>(512 + 4 * D) * 2))) return -2; h->emb_tmp = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->temb = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->ctemb = static_cast<bf16*>(p);
@@ -1179,6 +1407,17 @@ static int check_ready(rf_dit* h, const char* who, cudaStream_t s) {
     return -1;
   }
   if (rf_dit_missing_weights(h) != 0) return -4;
+  // an always target set after rf_dit_prepare puts a LoRA on rows the workspace may not cover yet
+  const int rows = lora_rows_needed(h, h->flags, h->N, h->n_cond);
+  if (rows > h->lora_rows) {
+    drop_graph(h);
+    for (bf16* old : {h->LT, h->LL}) {
+      auto it = std::find(h->geo_allocs.begin(), h->geo_allocs.end(), static_cast<void*>(old));
+      if (it != h->geo_allocs.end()) h->geo_allocs.erase(it);
+      cudaFree(old);
+    }
+    RF_TRY(alloc_lora_ws(h, rows));
+  }
   // fuse_lora mode: weights or adapters changed since the last merge -> re-merge before use
   h->use_merged = wants_merged(h, h->n_cond);
   if (h->use_merged && !merged_current(h)) {

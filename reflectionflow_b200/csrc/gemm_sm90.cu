@@ -707,7 +707,10 @@ int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT
   GemmGroupArgs g;
   memset(&g, 0, sizeof(g));
   g.A = X; g.lda = ldx; g.M = M; g.W = A; g.out = T; g.ldo = ldT;
-  return gemm_launch_impl(EPI_BIAS, NT, K, 1, &g, "lora_down", stream);
+  return lora_down_launch(K, NT, 1, &g, stream);
+}
+int lora_down_launch(int K, int NT, int ngroups, const GemmGroupArgs* groups, cudaStream_t stream) {
+  return gemm_launch_impl(EPI_BIAS, NT, K, ngroups, groups, "lora_down", stream);
 }
 
 // 3x3 (taps = 9) or 1x1 (taps = 1) convolution, stride 1 (zero padding 1) or stride 2 (diffusers

@@ -115,6 +115,10 @@ bool gemm_lora_eligible(int epi, int N, int K, const GemmGroupArgs& a);
 // on the GEMM kernel above (fp32 accumulation over the whole K, one rounding).
 int lora_down_launch(const bf16* X, int ldx, int M, int K, const bf16* A, int NT, bf16* T, int ldT,
                      cudaStream_t stream);
+// The same for up to 3 token streams in one launch, each group with its own rows (A, lda, M), its own A factor
+// (W: [NT, K]) and its own T (out, ldo): e.g. the text rows with the text stream's factors and the image + condition
+// rows with the shared ones.  bias, epilogue and LoRA fields of the groups must be zero.
+int lora_down_launch(int K, int NT, int ngroups, const GemmGroupArgs* groups, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------- attention
 // Non-causal softmax(Q K^T / sqrt(128)) V over one joint token sequence.

@@ -170,6 +170,10 @@ class B200FluxPipeline:
             lora = load_file(lora)
         self.transformer.load_lora(lora, alpha)
 
+    def unload_lora_weights(self):
+        """pipe.unload_lora_weights() (commented out at tts_reflectionflow.py:507): every LoRA target is unset."""
+        self.transformer.unload_lora()
+
     def set_adapters(self, *a, **k):
         pass
 

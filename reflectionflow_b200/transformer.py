@@ -222,6 +222,15 @@ class B200FluxTransformer2DModel:
             torch.cuda.synchronize(self.device)
         return self
 
+    def unload_lora(self):
+        """Unset every LoRA target (diffusers' unload_lora_weights): the model computes without an adapter until
+        load_lora is called again.  load_lora itself only adds or replaces targets, so switching from an adapter
+        on more modules to one on fewer goes through here."""
+        L.check(self._lib.rf_dit_clear_lora(self._h), "rf_dit_clear_lora")
+        self._geom_key = None  # the LoRA workspace, merged copies and captured step follow the new adapter set
+        self.has_lora = False
+        return self
+
     def set_lora_scale(self, scale: float):
         """diffusers' LoRA strength (joint_attention_kwargs["scale"]): multiplies every adapter's alpha / r from
         the next call on, until set again (1 = as loaded).  A captured denoise step built for another scale is

@@ -376,8 +376,12 @@ def build_pipeline(config: dict, args, ctx: DistCtx):
     return pipe
 
 
-def synthetic_lora(cfg, rank: int = 32, seed: int = 1):
-    """Random LoRA factors on the target list of train_flux/config.yaml:53."""
+def synthetic_lora(cfg, rank: int = 32, seed: int = 1, targets: str = "config"):
+    """Random LoRA factors on the target list of train_flux/config.yaml:53 (targets="config"), or on every Linear of
+    the transformer (targets="all-linear", train/model.py:73-80).  The config.yaml:53 factors are the same either
+    way: the other Linears draw afterwards from the same generator."""
+    if targets not in ("config", "all-linear"):
+        raise ValueError(f"targets must be 'config' or 'all-linear', got {targets!r}")
     d = cfg.inner_dim
     g = torch.Generator().manual_seed(seed)
     out = {}
@@ -399,6 +403,26 @@ def synthetic_lora(cfg, rank: int = 32, seed: int = 1):
         add(p + "proj_out", d, 5 * d)
         for n in ("attn.to_q", "attn.to_k", "attn.to_v"):
             add(p + n, d, d)
+    if targets == "all-linear":
+        add("context_embedder", d, cfg.joint_attention_dim)
+        tte = "time_text_embed."
+        add(tte + "timestep_embedder.linear_1", d, 256)
+        add(tte + "timestep_embedder.linear_2", d, d)
+        if cfg.guidance_embeds:
+            add(tte + "guidance_embedder.linear_1", d, 256)
+            add(tte + "guidance_embedder.linear_2", d, d)
+        add(tte + "text_embedder.linear_1", d, cfg.pooled_projection_dim)
+        add(tte + "text_embedder.linear_2", d, d)
+        for i in range(cfg.num_layers):
+            p = f"transformer_blocks.{i}."
+            add(p + "norm1_context.linear", 6 * d, d)
+            for n in ("attn.add_q_proj", "attn.add_k_proj", "attn.add_v_proj", "attn.to_add_out"):
+                add(p + n, d, d)
+            add(p + "ff.net.0.proj", 4 * d, d)
+            add(p + "ff_context.net.0.proj", 4 * d, d)
+            add(p + "ff_context.net.2", d, 4 * d)
+        add("norm_out.linear", 2 * d, d)
+        add("proj_out", cfg.in_channels, d)
     return out
 
 
