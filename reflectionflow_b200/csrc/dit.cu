@@ -28,8 +28,6 @@
 #include "rf_internal.h"
 
 namespace rf {
-int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R, float scale,
-                      cudaStream_t stream);
 int add2_launch(const bf16* a, const bf16* b, bf16* out, int n, cudaStream_t stream);
 int select_row_launch(const bf16* table, int64_t row_elems, const int* row, bf16* out,
                       cudaStream_t stream);

@@ -59,6 +59,98 @@ extern "C" {
 // test hook: 1 = the next GEMM launches use tiles at most 128 wide (covers both tile widths at small shapes)
 void rf_dbg_force_gemm_v1(int on) { rf::dbg_force_gemm_v1(on != 0); }
 
+// Test hooks over the internal launchers the DiT orchestrator calls (not declared in include/rf_b200.h): the grouped
+// GEMM with every epilogue and the fused LoRA fields, the grouped LoRA down-projection, the grouped LayerNorm +
+// modulate, the adaLN / embedder LoRA add and the fuse_lora merge.  rf_dbg_gemm_group mirrors rf::GemmGroupArgs
+// field by field; rf_dbg_gemm_group_size() lets a binding check its copy of the layout.
+struct rf_dbg_gemm_group {
+  const void* A; int lda; int M;
+  const void* W;
+  const void* bias;
+  void* out; int ldo;
+  const void* addend; int ldadd;
+  const void* res; int ldr;
+  const void* gate;
+  const float* rope_cos;
+  const float* rope_sin;
+  const void* norm_q;
+  const void* norm_k;
+  const void* lora_T; int ld_t;
+  const void* lora_B;
+  int lora_sec_cols;
+  int lora_pad;
+  float lora_scale[3];
+};
+
+size_t rf_dbg_gemm_group_size(void) { return sizeof(rf_dbg_gemm_group); }
+
+static int dbg_groups(int ngroups, const rf_dbg_gemm_group* src, rf::GemmGroupArgs* dst) {
+  if (!src || ngroups < 1 || ngroups > 3) {
+    rf::set_error("rf_dbg: 1..3 groups");
+    return -1;
+  }
+  memset(dst, 0, 3 * sizeof(rf::GemmGroupArgs));
+  for (int i = 0; i < ngroups; ++i) {
+    const rf_dbg_gemm_group& s = src[i];
+    rf::GemmGroupArgs& d = dst[i];
+    d.A = static_cast<const bf16*>(s.A); d.lda = s.lda; d.M = s.M;
+    d.W = static_cast<const bf16*>(s.W);
+    d.bias = static_cast<const bf16*>(s.bias);
+    d.out = static_cast<bf16*>(s.out); d.ldo = s.ldo;
+    d.addend = static_cast<const bf16*>(s.addend); d.ldadd = s.ldadd;
+    d.res = static_cast<const bf16*>(s.res); d.ldr = s.ldr;
+    d.gate = static_cast<const bf16*>(s.gate);
+    d.rope_cos = s.rope_cos; d.rope_sin = s.rope_sin;
+    d.norm_q = static_cast<const bf16*>(s.norm_q);
+    d.norm_k = static_cast<const bf16*>(s.norm_k);
+    d.lora_T = static_cast<const bf16*>(s.lora_T); d.ld_t = s.ld_t;
+    d.lora_B = static_cast<const bf16*>(s.lora_B);
+    d.lora_sec_cols = s.lora_sec_cols;
+    d.lora_pad = s.lora_pad;
+    for (int k = 0; k < 3; ++k) d.lora_scale[k] = s.lora_scale[k];
+  }
+  return 0;
+}
+
+int rf_dbg_gemm_grouped(int epi, int N, int K, int ngroups, const rf_dbg_gemm_group* g, void* stream) {
+  rf::GemmGroupArgs a[3];
+  if (int rc = dbg_groups(ngroups, g, a)) return rc;
+  return rf::gemm_launch(epi, N, K, ngroups, a, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_lora_down_grouped(int K, int NT, int ngroups, const rf_dbg_gemm_group* g, void* stream) {
+  rf::GemmGroupArgs a[3];
+  if (int rc = dbg_groups(ngroups, g, a)) return rc;
+  return rf::lora_down_launch(K, NT, ngroups, a, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_ln_modulate_grouped(const void* x, int ldx, void* out, int ldo, int dim, int ngroups, const int* row_end,
+                               const void* const* scale, const void* const* shift, void* stream) {
+  if (!x || !out || !row_end || !scale || !shift || ngroups < 1 || ngroups > 3) {
+    rf::set_error("rf_dbg_ln_modulate_grouped: null operand or not 1..3 groups");
+    return -1;
+  }
+  const bf16* sc[3] = {nullptr, nullptr, nullptr};
+  const bf16* sh[3] = {nullptr, nullptr, nullptr};
+  for (int i = 0; i < ngroups; ++i) {
+    sc[i] = static_cast<const bf16*>(scale[i]);
+    sh[i] = static_cast<const bf16*>(shift[i]);
+  }
+  return rf::ln_modulate_grouped_launch(static_cast<const bf16*>(x), ldx, static_cast<bf16*>(out), ldo, dim, ngroups,
+                                        row_end, sc, sh, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_add_rows(void* dst, int64_t ldd, const void* src, int lds, int rows, int cols, float scale, void* stream) {
+  return rf::add_rows_launch(static_cast<bf16*>(dst), ldd, static_cast<const bf16*>(src), lds, rows, cols, scale,
+                             static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_lora_merge(const void* W, const void* A, const void* B, void* Wm, int N, int K, int R, float scale,
+                      void* stream) {
+  return rf::lora_merge_launch(static_cast<const bf16*>(W), static_cast<const bf16*>(A), static_cast<const bf16*>(B),
+                               static_cast<bf16*>(Wm), N, K, R, scale, static_cast<cudaStream_t>(stream));
+}
+
 
 const char* rf_last_error(void) { return rf::get_error(); }
 int rf_abi_version(void) { return RF_B200_ABI_VERSION; }

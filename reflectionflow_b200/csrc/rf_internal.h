@@ -171,5 +171,8 @@ int copy_rows_launch(const bf16* src, int lds, bf16* dst, int ldd, int rows, int
 // dst[r * ldd + c] = bf16(dst[r * ldd + c] + bf16(src[r * lds + c] * scale)) for r < rows, c < cols
 int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, int cols, float scale,
                     cudaStream_t stream);
+// Wm[n, k] = bf16(W[n, k] + scale * sum_r B[n, r] A[r, k]) (peft's merged weight; W, Wm [N, K], A [R, K], B [N, R])
+int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R, float scale,
+                      cudaStream_t stream);
 
 }  // namespace rf

@@ -192,25 +192,16 @@ def _call_linear_lora(epi, x, W, bias, y, Ap, Bp, t_cols, res=None, gate=None, c
     M, K = x.shape
     N = W.shape[0]
     ws = torch.zeros(lib.rf_op_linear_lora_workspace_bytes(M), dtype=torch.uint8, device=_dev())
-    for _ in range(2):  # twice: the in-kernel split-K counters must re-arm themselves
-        rc = lib.rf_op_linear_lora(epi, M, N, K, L.ptr(x), x.stride(0), L.ptr(W), L.ptr(bias), L.ptr(y), y.stride(0),
-                                   L.ptr(Ap), t_cols, L.ptr(Bp), L.ptr(res), res.stride(0) if res is not None else 0,
-                                   L.ptr(gate), L.ptr(cos), L.ptr(sin), L.ptr(nq), L.ptr(nk), L.ptr(ws), L.cur_stream())
-        L.check(rc, "rf_op_linear_lora")
+    rc = lib.rf_op_linear_lora(epi, M, N, K, L.ptr(x), x.stride(0), L.ptr(W), L.ptr(bias), L.ptr(y), y.stride(0),
+                               L.ptr(Ap), t_cols, L.ptr(Bp), L.ptr(res), res.stride(0) if res is not None else 0,
+                               L.ptr(gate), L.ptr(cos), L.ptr(sin), L.ptr(nq), L.ptr(nk), L.ptr(ws), L.cur_stream())
+    L.check(rc, "rf_op_linear_lora")
     torch.cuda.synchronize()
 
 
-@pytest.fixture(params=["split", "side"])
-def lora_down_form(request, monkeypatch):
-    """both forms of T = bf16(x A^T): the chip-filling launch and the confined few-CTA launch that the DiT forks beside
-    its main GEMM (csrc/gemm_sm90.cu); the op reads RF_LORA_DOWN at call time"""
-    monkeypatch.setenv("RF_LORA_DOWN", request.param)
-    return request.param
-
-
 @pytest.mark.parametrize("M,N,K", [(1024, 3072, 3072), (1024, 3072, 15360), (256, 256, 256), (1000, 1024, 12288)])
-def test_linear_lora_gate_res(M, N, K, lora_down_form):
-    """fused peft-LoRA GEMM (split-K down-projection + low-rank k-block in the main GEMM) at the
+def test_linear_lora_gate_res(M, N, K):
+    """fused peft-LoRA GEMM (down-projection GEMM + low-rank k-block in the main GEMM) at the
     headline condition-stream shapes: to_out / ff.net.2 / single proj_out (lora_controller.py:5-42)"""
     x = _randn(M, K, seed=70)
     W = _randn(N, K, scale=1.0 / math.sqrt(K), seed=71)
@@ -229,7 +220,7 @@ def test_linear_lora_gate_res(M, N, K, lora_down_form):
     assert (y == ref).float().mean().item() > 0.98
 
 
-def test_linear_lora_gelu(lora_down_form):
+def test_linear_lora_gelu():
     M, N, K = 1024, 12288, 3072
     x = _randn(M, K, seed=80)
     W = _randn(N, K, scale=1.0 / math.sqrt(K), seed=81)
@@ -247,7 +238,7 @@ def test_linear_lora_gelu(lora_down_form):
 
 
 @pytest.mark.parametrize("M,heads,K,only", [(1024, 24, 3072, None), (384, 2, 256, None), (1024, 2, 256, "k")])
-def test_linear_lora_qkv(M, heads, K, only, lora_down_form):
+def test_linear_lora_qkv(M, heads, K, only):
     """stacked q|k|v with per-section adapters (only="k": a k-only adapter — q and v get a zero term)"""
     D = heads * 128
     N = 3 * D
