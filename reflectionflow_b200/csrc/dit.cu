@@ -58,44 +58,43 @@ struct Lin {  // views into the weight arena
   bf16* b = nullptr;
 };
 
-struct LoraT {  // factors of one target, rank zero-padded to the handle's lora_pad
-  bf16* A = nullptr;  // [lora_pad, in]
-  bf16* B = nullptr;  // [out, lora_pad]
+struct LoraPack;
+struct LoraT {  // one target Linear of an adapter
   int in = 0, out = 0;
   bool set = false;
   double scale = 1.0;  // lora_alpha / r
-  // The Linears outside train_flux/config.yaml:53 (text stream, embedders, final layer, ff.net.0.proj) are "always"
-  // targets: no enable_lora block names them, so every call applies them, latent_lora or not.  Their factors are
-  // allocated on the first rf_dit_set_lora, so a handle that never sees such an adapter keeps its footprint.  A
-  // member of a stacked pack (add_q|k|v) allocates the whole pack, zeroed, and points its siblings into it.
-  bool always = false;
-  LoraT* pack[3] = {nullptr, nullptr, nullptr};
-  int npack = 0;
-  bf16** packA = nullptr;
-  bf16** packB = nullptr;
+  LoraPack* pack = nullptr;
+  int slot = 0;  // its factors are slot `slot` of the pack's stacked A / B
 };
-// (merged weights W + B A of a whole packed projection live in the block structs: *_m)
+
+// The adapter of one packed weight: 1 target, or the 3 stacked q|k|v ones, with factors zero-padded to the handle's
+// lora_pad.  The Linears of train_flux/config.yaml:53 are gated by enable_lora / latent_lora; the others (text
+// stream, embedders, final layer, ff.net.0.proj) are "always" packs: no enable_lora block names them, so they apply
+// to every row that reads their weight.  Factors of the gated packs are allocated at create, those of the always
+// packs on their first rf_dit_set_lora (lora_storage), so a handle that never sees such an adapter keeps its footprint.
+struct LoraPack {
+  LoraT t[3];
+  int n = 0;
+  bool always = false;
+  bf16* A = nullptr;        // [n lora_pad, in]
+  bf16* B = nullptr;        // [n out, lora_pad] (rows of the packed projection)
+  const bf16* W = nullptr;  // base weight [n out, in] of a projection (nullptr: a GEMV target, never merged)
+  bf16* Wm = nullptr;       // merged W + s B A (fuse_lora mode), allocated on the first merge with a target set
+};
+bf16* lora_A(const LoraT& t, int pad) { return t.pack->A + static_cast<int64_t>(t.slot) * pad * t.in; }
+bf16* lora_B(const LoraT& t, int pad) { return t.pack->B + static_cast<int64_t>(t.slot) * t.out * pad; }
 
 struct DoubleBlk {
   Lin qkv, add_qkv, to_out, to_add_out, ff1, ff2, ffc1, ffc2;
   bf16 *norm_q, *norm_k, *norm_added_q, *norm_added_k;
-  LoraT l_norm1, l_q, l_k, l_v, l_out, l_ff2;
-  // always targets: text stream (norm1_context, add_q|k|v, to_add_out, ff_context) and ff.net.0.proj
-  LoraT l_norm1c, l_aq, l_ak, l_av, l_add_out, l_ff1, l_ffc1, l_ffc2;
-  bf16* qkvA = nullptr;  // [3 lora_pad, D] = stacked A of to_q/to_k/to_v
-  bf16* qkvB = nullptr;  // [3D, lora_pad] = stacked B (rows of the packed q|k|v projection)
-  bf16* add_qkvA = nullptr;  // the same for add_q_proj / add_k_proj / add_v_proj (allocated on first use)
-  bf16* add_qkvB = nullptr;
-  bf16 *qkv_m = nullptr, *to_out_m = nullptr, *ff2_m = nullptr;  // merged W + B A (fuse_lora mode)
-  bf16 *add_qkv_m = nullptr, *to_add_out_m = nullptr, *ff1_m = nullptr, *ffc1_m = nullptr, *ffc2_m = nullptr;
+  LoraPack l_norm1, l_qkv, l_out, l_ff2;
+  // always: text stream (norm1_context, add_q|k|v, to_add_out, ff_context) and ff.net.0.proj
+  LoraPack l_norm1c, l_add_qkv, l_add_out, l_ff1, l_ffc1, l_ffc2;
 };
 struct SingleBlk {
   Lin qkv, mlp, out;
   bf16 *norm_q, *norm_k;
-  LoraT l_norm, l_q, l_k, l_v, l_mlp, l_out;
-  bf16* qkvA = nullptr;
-  bf16* qkvB = nullptr;
-  bf16 *qkv_m = nullptr, *mlp_m = nullptr, *out_m = nullptr;
+  LoraPack l_norm, l_qkv, l_mlp, l_out;
 };
 
 }  // namespace
@@ -110,9 +109,10 @@ struct rf_dit {
   std::unordered_map<std::string, Slot> slots;
   std::unordered_map<std::string, LoraT*> lora_slots;
   Lin x_emb, ctx_emb, t1, t2, g1, g2, p1, p2, proj_out;
-  LoraT l_x_emb;
-  // always targets at the top level: context_embedder, the time / guidance / text embedders, norm_out, proj_out
-  LoraT l_ctx, l_t1, l_t2, l_g1, l_g2, l_p1, l_p2, l_norm_out, l_proj_out;
+  LoraPack l_x_emb;
+  // always packs at the top level: context_embedder, the time / guidance / text embedders, norm_out, proj_out
+  LoraPack l_ctx, l_t1, l_t2, l_g1, l_g2, l_p1, l_p2, l_norm_out, l_proj_out;
+  std::vector<LoraPack*> proj_packs;  // the packs of every projection (merge_all)
   bf16* modW = nullptr;
   bf16* modB = nullptr;
   int64_t n_mod = 0;
@@ -128,8 +128,6 @@ struct rf_dit {
   bool lora_merged = false;   // merged copies are current for merged_call_scale
   double merged_call_scale = 1.0;
   bool use_merged = false;    // rf_dit_prepare flag bit 3
-  bf16* x_emb_m = nullptr;
-  bf16 *ctx_emb_m = nullptr, *proj_out_m = nullptr;
   // ---- geometry
   bool prepared = false;
   int batch = 0, n_txt = 0, n_img = 0, n_cond = 0, N = 0, n_main = 0;
@@ -139,10 +137,9 @@ struct rf_dit {
   float *rope_cos = nullptr, *rope_sin = nullptr, *crope_cos = nullptr, *crope_sin = nullptr;
   // ---- workspace
   bf16 *X = nullptr, *XN = nullptr, *QKV = nullptr, *ACT = nullptr, *MOD = nullptr, *MODC = nullptr;
-  bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [lora_rows, 256], L [lora_rows, 4D]
+  bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [lora_rows, 4 lora_pad], L [lora_rows, 4D]
   int lora_rows = 0;
-  bf16 *emb_tmp = nullptr;            // small vectors for the temb path
-  bf16 *temb = nullptr, *ctemb = nullptr;
+  bf16* emb_ws = nullptr;             // temb_mod workspace of one vector (eager step, cond_temb)
   // ---- staging for the graph-captured denoise loop
   bf16 *s_lat = nullptr, *s_txt = nullptr, *s_pooled = nullptr, *s_cond = nullptr, *s_v = nullptr;
   bf16 *s_tsteps = nullptr, *s_guid = nullptr, *s_zero_one = nullptr;
@@ -200,52 +197,36 @@ Lin new_lin(rf_dit* h, Arena& ar, const std::string& mod, int out, int in) {
   return l;
 }
 
-void new_lora(rf_dit* h, Arena& ar, const std::string& mod, LoraT& t, int out, int in,
-              bf16* A_view = nullptr, bf16* B_view = nullptr) {
-  if (h->cfg.lora_rank <= 0) return;
-  t.in = in;
-  t.out = out;
-  const int pad = h->lora_pad;
-  t.A = A_view ? A_view : ar.take(static_cast<int64_t>(pad) * in);
-  t.B = B_view ? B_view : ar.take(static_cast<int64_t>(out) * pad);
-  // unset targets must contribute exactly zero (a q-only adapter still runs the stacked q|k|v path)
-  if (t.A) cudaMemset(t.A, 0, static_cast<size_t>(pad) * in * 2);
-  if (t.B) cudaMemset(t.B, 0, static_cast<size_t>(out) * pad * 2);
-  h->lora_slots[mod] = &t;
-}
-
-// an always target: shape checks now, factor storage on its first rf_dit_set_lora (lora_storage)
-void new_always_lora(rf_dit* h, const std::string& mod, LoraT& t, int out, int in) {
-  if (h->cfg.lora_rank <= 0) return;
-  t.in = in;
-  t.out = out;
-  t.always = true;
-  h->lora_slots[mod] = &t;
-}
-
-// zeroed factor storage of target t (of its whole pack), allocated on first use; live until destroy
-int lora_storage(rf_dit* h, LoraT& t) {
-  if (t.A != nullptr) return 0;
-  const int64_t pad = h->lora_pad, n = t.npack ? t.npack : 1;
-  const int64_t a_elems = pad * t.in, b_elems = static_cast<int64_t>(t.out) * pad;
-  void *pa = nullptr, *pb = nullptr;
-  RF_TRY(dev_alloc(h, &pa, static_cast<size_t>(n * a_elems) * 2));
-  RF_TRY(dev_alloc(h, &pb, static_cast<size_t>(n * b_elems) * 2));
-  RF_CHECK_CUDA(cudaMemset(pa, 0, static_cast<size_t>(n * a_elems) * 2));
-  RF_CHECK_CUDA(cudaMemset(pb, 0, static_cast<size_t>(n * b_elems) * 2));
-  bf16 *A = static_cast<bf16*>(pa), *B = static_cast<bf16*>(pb);
-  if (t.npack == 0) {
-    t.A = A;
-    t.B = B;
-    return 0;
+// Zeroed factor storage of pack p, live until destroy: unset members must add exactly nothing (a q-only adapter
+// still runs the stacked q|k|v path).  A preset A is a view into a larger stack and is only zeroed.
+int lora_storage(rf_dit* h, LoraPack& p) {
+  if (p.B != nullptr) return 0;
+  const size_t a = static_cast<size_t>(p.n) * h->lora_pad * p.t[0].in * 2;
+  const size_t b = static_cast<size_t>(p.n) * p.t[0].out * h->lora_pad * 2;
+  void* q = nullptr;
+  if (p.A == nullptr) {
+    RF_TRY(dev_alloc(h, &q, a));
+    p.A = static_cast<bf16*>(q);
   }
-  *t.packA = A;
-  *t.packB = B;
-  for (int k = 0; k < t.npack; ++k) {
-    t.pack[k]->A = A + k * a_elems;
-    t.pack[k]->B = B + k * b_elems;
-  }
+  RF_TRY(dev_alloc(h, &q, b));
+  p.B = static_cast<bf16*>(q);
+  RF_CHECK_CUDA(cudaMemset(p.A, 0, a));
+  RF_CHECK_CUDA(cudaMemset(p.B, 0, b));
   return 0;
+}
+
+// the pack of the targets `mods`, each out x in and stacked in that order; W: the packed projection weight
+void new_pack(rf_dit* h, Arena& ar, LoraPack& p, std::initializer_list<std::string> mods, int out, int in,
+              const bf16* W, bool always) {
+  if (h->cfg.lora_rank <= 0) return;
+  for (const std::string& m : mods) {
+    p.t[p.n] = LoraT{in, out, false, 1.0, &p, p.n};
+    h->lora_slots[m] = &p.t[p.n++];
+  }
+  p.always = always;
+  p.W = W;
+  if (W) h->proj_packs.push_back(&p);
+  if (!always && lora_storage(h, p)) ar.fail = -2;
 }
 
 int build_storage(rf_dit* h) {
@@ -253,26 +234,26 @@ int build_storage(rf_dit* h) {
   const int D = h->D, lpad = h->lora_pad;
   Arena ar{h};
   h->x_emb = new_lin(h, ar, "x_embedder", D, c.in_channels);
-  new_lora(h, ar, "x_embedder", h->l_x_emb, D, c.in_channels);
+  new_pack(h, ar, h->l_x_emb, {"x_embedder"}, D, c.in_channels, h->x_emb.w, false);
   h->ctx_emb = new_lin(h, ar, "context_embedder", D, c.joint_attention_dim);
-  new_always_lora(h, "context_embedder", h->l_ctx, D, c.joint_attention_dim);
+  new_pack(h, ar, h->l_ctx, {"context_embedder"}, D, c.joint_attention_dim, h->ctx_emb.w, true);
   const std::string tte = "time_text_embed.";
   h->t1 = new_lin(h, ar, tte + "timestep_embedder.linear_1", D, 256);
   h->t2 = new_lin(h, ar, tte + "timestep_embedder.linear_2", D, D);
-  new_always_lora(h, tte + "timestep_embedder.linear_1", h->l_t1, D, 256);
-  new_always_lora(h, tte + "timestep_embedder.linear_2", h->l_t2, D, D);
+  new_pack(h, ar, h->l_t1, {tte + "timestep_embedder.linear_1"}, D, 256, nullptr, true);
+  new_pack(h, ar, h->l_t2, {tte + "timestep_embedder.linear_2"}, D, D, nullptr, true);
   if (c.guidance_embeds) {
     h->g1 = new_lin(h, ar, tte + "guidance_embedder.linear_1", D, 256);
     h->g2 = new_lin(h, ar, tte + "guidance_embedder.linear_2", D, D);
-    new_always_lora(h, tte + "guidance_embedder.linear_1", h->l_g1, D, 256);
-    new_always_lora(h, tte + "guidance_embedder.linear_2", h->l_g2, D, D);
+    new_pack(h, ar, h->l_g1, {tte + "guidance_embedder.linear_1"}, D, 256, nullptr, true);
+    new_pack(h, ar, h->l_g2, {tte + "guidance_embedder.linear_2"}, D, D, nullptr, true);
   }
   h->p1 = new_lin(h, ar, tte + "text_embedder.linear_1", D, c.pooled_projection_dim);
   h->p2 = new_lin(h, ar, tte + "text_embedder.linear_2", D, D);
-  new_always_lora(h, tte + "text_embedder.linear_1", h->l_p1, D, c.pooled_projection_dim);
-  new_always_lora(h, tte + "text_embedder.linear_2", h->l_p2, D, D);
+  new_pack(h, ar, h->l_p1, {tte + "text_embedder.linear_1"}, D, c.pooled_projection_dim, nullptr, true);
+  new_pack(h, ar, h->l_p2, {tte + "text_embedder.linear_2"}, D, D, nullptr, true);
   h->proj_out = new_lin(h, ar, "proj_out", c.in_channels, D);
-  new_always_lora(h, "proj_out", h->l_proj_out, c.in_channels, D);
+  new_pack(h, ar, h->l_proj_out, {"proj_out"}, c.in_channels, D, h->proj_out.w, true);
 
   h->n_mod = static_cast<int64_t>(c.num_layers) * 12 * D +
              static_cast<int64_t>(c.num_single_layers) * 3 * D + 2 * D;
@@ -286,47 +267,36 @@ int build_storage(rf_dit* h) {
     const int64_t mo = static_cast<int64_t>(i) * 12 * D;
     reg_lin(h, p + "norm1.linear", h->modW + mo * D, h->modB + mo, 6 * D, D);
     reg_lin(h, p + "norm1_context.linear", h->modW + (mo + 6 * D) * D, h->modB + mo + 6 * D, 6 * D, D);
-    new_lora(h, ar, p + "norm1.linear", b.l_norm1, 6 * D, D);
-    new_always_lora(h, p + "norm1_context.linear", b.l_norm1c, 6 * D, D);
+    new_pack(h, ar, b.l_norm1, {p + "norm1.linear"}, 6 * D, D, nullptr, false);
+    new_pack(h, ar, b.l_norm1c, {p + "norm1_context.linear"}, 6 * D, D, nullptr, true);
     b.qkv = new_lin(h, ar, "", 3 * D, D);
     b.add_qkv = new_lin(h, ar, "", 3 * D, D);
     const char* nm[3] = {"to_q", "to_k", "to_v"};
     const char* an[3] = {"add_q_proj", "add_k_proj", "add_v_proj"};
-    if (c.lora_rank > 0) {
-      b.qkvA = ar.take(static_cast<int64_t>(3 * lpad) * D);
-      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * lpad);
-    }
-    LoraT* lq[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraT* la[3] = {&b.l_aq, &b.l_ak, &b.l_av};
     for (int j = 0; j < 3; ++j) {
       reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
       reg_lin(h, p + "attn." + an[j], b.add_qkv.w + static_cast<int64_t>(j) * D * D,
               b.add_qkv.b + j * D, D, D);
-      new_lora(h, ar, p + "attn." + nm[j], *lq[j], D, D,
-               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * lpad * D : nullptr,
-               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * lpad : nullptr);
-      new_always_lora(h, p + "attn." + an[j], *la[j], D, D);
-      la[j]->npack = 3;
-      la[j]->packA = &b.add_qkvA;
-      la[j]->packB = &b.add_qkvB;
-      for (int k = 0; k < 3; ++k) la[j]->pack[k] = la[k];
     }
+    new_pack(h, ar, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false);
+    new_pack(h, ar, b.l_add_qkv, {p + "attn.add_q_proj", p + "attn.add_k_proj", p + "attn.add_v_proj"}, D, D,
+             b.add_qkv.w, true);
     b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
     b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
     b.norm_added_q = ar.take(128); reg(h, p + "attn.norm_added_q.weight", b.norm_added_q, 128);
     b.norm_added_k = ar.take(128); reg(h, p + "attn.norm_added_k.weight", b.norm_added_k, 128);
     b.to_out = new_lin(h, ar, p + "attn.to_out.0", D, D);
-    new_lora(h, ar, p + "attn.to_out.0", b.l_out, D, D);
+    new_pack(h, ar, b.l_out, {p + "attn.to_out.0"}, D, D, b.to_out.w, false);
     b.to_add_out = new_lin(h, ar, p + "attn.to_add_out", D, D);
-    new_always_lora(h, p + "attn.to_add_out", b.l_add_out, D, D);
+    new_pack(h, ar, b.l_add_out, {p + "attn.to_add_out"}, D, D, b.to_add_out.w, true);
     b.ff1 = new_lin(h, ar, p + "ff.net.0.proj", 4 * D, D);
-    new_always_lora(h, p + "ff.net.0.proj", b.l_ff1, 4 * D, D);
+    new_pack(h, ar, b.l_ff1, {p + "ff.net.0.proj"}, 4 * D, D, b.ff1.w, true);
     b.ff2 = new_lin(h, ar, p + "ff.net.2", D, 4 * D);
-    new_lora(h, ar, p + "ff.net.2", b.l_ff2, D, 4 * D);
+    new_pack(h, ar, b.l_ff2, {p + "ff.net.2"}, D, 4 * D, b.ff2.w, false);
     b.ffc1 = new_lin(h, ar, p + "ff_context.net.0.proj", 4 * D, D);
     b.ffc2 = new_lin(h, ar, p + "ff_context.net.2", D, 4 * D);
-    new_always_lora(h, p + "ff_context.net.0.proj", b.l_ffc1, 4 * D, D);
-    new_always_lora(h, p + "ff_context.net.2", b.l_ffc2, D, 4 * D);
+    new_pack(h, ar, b.l_ffc1, {p + "ff_context.net.0.proj"}, 4 * D, D, b.ffc1.w, true);
+    new_pack(h, ar, b.l_ffc2, {p + "ff_context.net.2"}, D, 4 * D, b.ffc2.w, true);
   }
   h->sgl.resize(c.num_single_layers);
   const int64_t so = static_cast<int64_t>(c.num_layers) * 12 * D;
@@ -335,33 +305,28 @@ int build_storage(rf_dit* h) {
     const std::string p = "single_transformer_blocks." + std::to_string(i) + ".";
     const int64_t mo = so + static_cast<int64_t>(i) * 3 * D;
     reg_lin(h, p + "norm.linear", h->modW + mo * D, h->modB + mo, 3 * D, D);
-    new_lora(h, ar, p + "norm.linear", b.l_norm, 3 * D, D);
+    new_pack(h, ar, b.l_norm, {p + "norm.linear"}, 3 * D, D, nullptr, false);
     b.qkv = new_lin(h, ar, "", 3 * D, D);
+    const char* nm[3] = {"to_q", "to_k", "to_v"};
+    for (int j = 0; j < 3; ++j)
+      reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
+    b.mlp = new_lin(h, ar, p + "proj_mlp", 4 * D, D);
     if (c.lora_rank > 0) {
       // A factors of to_q | to_k | to_v | proj_mlp stacked: all four read the same normalised tokens, so
-      // ONE down-projection launch (NT = 256) serves the q|k|v and the MLP-in GEMMs of the block
-      b.qkvA = ar.take(static_cast<int64_t>(4 * lpad) * D);
-      b.qkvB = ar.take(static_cast<int64_t>(3 * D) * lpad);
+      // ONE down-projection launch (NT = 4 lora_pad) serves the q|k|v and the MLP-in GEMMs of the block
+      b.l_qkv.A = ar.take(static_cast<int64_t>(4 * lpad) * D);
+      b.l_mlp.A = b.l_qkv.A ? b.l_qkv.A + static_cast<int64_t>(3 * lpad) * D : nullptr;
     }
-    const char* nm[3] = {"to_q", "to_k", "to_v"};
-    LoraT* lq[3] = {&b.l_q, &b.l_k, &b.l_v};
-    for (int j = 0; j < 3; ++j) {
-      reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
-      new_lora(h, ar, p + "attn." + nm[j], *lq[j], D, D,
-               b.qkvA ? b.qkvA + static_cast<int64_t>(j) * lpad * D : nullptr,
-               b.qkvB ? b.qkvB + static_cast<int64_t>(j) * D * lpad : nullptr);
-    }
+    new_pack(h, ar, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false);
+    new_pack(h, ar, b.l_mlp, {p + "proj_mlp"}, 4 * D, D, b.mlp.w, false);
     b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
     b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
-    b.mlp = new_lin(h, ar, p + "proj_mlp", 4 * D, D);
-    new_lora(h, ar, p + "proj_mlp", b.l_mlp, 4 * D, D,
-             b.qkvA ? b.qkvA + static_cast<int64_t>(3 * lpad) * D : nullptr);
     b.out = new_lin(h, ar, p + "proj_out", D, 5 * D);
-    new_lora(h, ar, p + "proj_out", b.l_out, D, 5 * D);
+    new_pack(h, ar, b.l_out, {p + "proj_out"}, D, 5 * D, b.out.w, false);
   }
   const int64_t oo = so + static_cast<int64_t>(c.num_single_layers) * 3 * D;
   reg_lin(h, "norm_out.linear", h->modW + oo * D, h->modB + oo, 2 * D, D);
-  new_always_lora(h, "norm_out.linear", h->l_norm_out, 2 * D, D);
+  new_pack(h, ar, h->l_norm_out, {"norm_out.linear"}, 2 * D, D, nullptr, true);
   return ar.fail;
 }
 
@@ -387,67 +352,48 @@ int add_vec_lora(rf_dit* h, const LoraT& t, const bf16* x, int ldx, int batch, i
                  bf16* tvec, bf16* lvec, cudaStream_t s) {
   if (!lora_on(h, t)) return 0;
   const int lpad = h->lora_pad;
-  RF_TRY(rf::gemv_launch(x, ldx, batch, t.A, nullptr, tvec, lpad, lpad, t.in, act, s));
-  RF_TRY(rf::gemv_launch(tvec, lpad, batch, t.B, nullptr, lvec, t.out, t.out, lpad, 0, s));
+  RF_TRY(rf::gemv_launch(x, ldx, batch, lora_A(t, lpad), nullptr, tvec, lpad, lpad, t.in, act, s));
+  RF_TRY(rf::gemv_launch(tvec, lpad, batch, lora_B(t, lpad), nullptr, lvec, t.out, t.out, lpad, 0, s));
   return rf::add_rows_launch(y, ldy, lvec, t.out, batch, t.out, lora_eff(h, t), s);
 }
 
 // y = linear_2(silu(linear_1(x)))  (TimestepEmbedding / PixArtAlphaTextProjection) for `batch` vectors, each Linear
 // with its LoRA term (always targets): linear_2's sees the same bf16(silu(.)) input as its GEMV.
 // tvec [batch, lora_pad], lvec [batch, D] scratch.
-int mlp2(rf_dit* h, const bf16* x, int in_dim, int batch, const Lin& l1, const LoraT& lt1, const Lin& l2,
-         const LoraT& lt2, bf16* tmp, bf16* out, bf16* tvec, bf16* lvec, cudaStream_t s) {
+int mlp2(rf_dit* h, const bf16* x, int in_dim, int batch, const Lin& l1, const LoraPack& lp1, const Lin& l2,
+         const LoraPack& lp2, bf16* tmp, bf16* out, bf16* tvec, bf16* lvec, cudaStream_t s) {
   const int D = h->D;
   RF_TRY(rf::gemv_launch(x, in_dim, batch, l1.w, l1.b, tmp, D, D, in_dim, 0, s));
-  RF_TRY(add_vec_lora(h, lt1, x, in_dim, batch, 0, tmp, D, tvec, lvec, s));
+  RF_TRY(add_vec_lora(h, lp1.t[0], x, in_dim, batch, 0, tmp, D, tvec, lvec, s));
   RF_TRY(rf::gemv_launch(tmp, D, batch, l2.w, l2.b, out, D, D, D, 1, s));
-  return add_vec_lora(h, lt2, tmp, D, batch, 1, out, D, tvec, lvec, s);
+  return add_vec_lora(h, lp2.t[0], tmp, D, batch, 1, out, D, tvec, lvec, s);
 }
 
-// temb = time(t) + guidance(g) + text(pooled)   (CombinedTimestepGuidanceTextProjEmbeddings)
-int compute_temb(rf_dit* h, const bf16* t, const int* step, const bf16* guid, const bf16* pooled,
-                 bf16* out, cudaStream_t s) {
-  const int D = h->D;
-  bf16* e = h->emb_tmp;  // [256 | 256 | D tmp | D a | D b | D c]
-  bf16 *tp = e, *gp = e + 256, *tmp = e + 512, *a = tmp + D, *b = a + D, *c = b + D;
-  bf16 *tvec = h->LT, *lvec = h->LT + 256;  // embedder LoRA scratch: [lora_pad] | [D] (LT holds >= 8D)
-  RF_TRY(rf::timestep_embed_launch(t, step, 1, 1000.0f, tp, 1, s));
-  RF_TRY(mlp2(h, tp, 256, 1, h->t1, h->l_t1, h->t2, h->l_t2, tmp, a, tvec, lvec, s));
-  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, 1, h->p1, h->l_p1, h->p2, h->l_p2, tmp, c, tvec, lvec, s));
-  if (h->cfg.guidance_embeds) {
-    RF_TRY(rf::timestep_embed_launch(guid, nullptr, 1, 1000.0f, gp, 1, s));
-    RF_TRY(mlp2(h, gp, 256, 1, h->g1, h->l_g1, h->g2, h->l_g2, tmp, b, tvec, lvec, s));
-    RF_TRY(rf::add3_launch(a, b, c, out, D, s));
-  } else {
-    RF_TRY(rf::add2_launch(a, c, out, D, s));
-  }
-  return 0;
-}
-
-// L[rows, :] = bf16( bf16(x A^T) B^T ): the unfused peft low-rank term of `rows` tokens for n = 1 target, or for
-// the n = 3 stacked q|k|v targets (A_all = [Aq;Ak;Av]: T = x A_all^T in one GEMM, L[:, jD:(j+1)D] = T_j B_j^T
-// grouped).  T != nullptr: bf16(x A_all^T) of these rows was already computed (pitch ld_t); only the up-projection
-// runs.  Otherwise T is computed here into LT.
-int lora_term(rf_dit* h, const LoraT* const* ls, int n, const bf16* A_all, const bf16* x, int ldx, int rows,
-              const bf16* T, int ld_t, bf16* L, int ldl, cudaStream_t s) {
+// L[rows, :] = bf16( bf16(x A^T) B^T ): the unfused peft low-rank term of `rows` tokens for pack p (n = 1 target, or
+// the n = 3 stacked q|k|v targets: T = x A^T in one GEMM, L[:, jD:(j+1)D] = T_j B_j^T grouped).  T != nullptr:
+// bf16(x A^T) of these rows was already computed (pitch ld_t); only the up-projection runs.  Otherwise T is computed
+// here into LT.
+int lora_term(rf_dit* h, const LoraPack& p, const bf16* x, int ldx, int rows, const bf16* T, int ld_t, bf16* L,
+              int ldl, cudaStream_t s) {
   const int lpad = h->lora_pad;
   rf::GemmGroupArgs g[3];
   if (T == nullptr) {
     memset(g, 0, sizeof(g));
-    g[0].A = x; g[0].lda = ldx; g[0].M = rows; g[0].W = A_all; g[0].out = h->LT; g[0].ldo = n * lpad;
-    RF_TRY(rf::gemm_launch(rf::EPI_BIAS, n * lpad, ls[0]->in, 1, g, s));
+    g[0].A = x; g[0].lda = ldx; g[0].M = rows; g[0].W = p.A; g[0].out = h->LT; g[0].ldo = p.n * lpad;
+    RF_TRY(rf::gemm_launch(rf::EPI_BIAS, p.n * lpad, p.t[0].in, 1, g, s));
     T = h->LT;
-    ld_t = n * lpad;
+    ld_t = p.n * lpad;
   }
   memset(g, 0, sizeof(g));
   bool scaled = false;  // peft's bf16(bf16(T B^T) * scaling): the scale is the up-projection's output scale
-  for (int j = 0; j < n; ++j) {
+  for (int j = 0; j < p.n; ++j) {
+    const LoraT& t = p.t[j];
     g[j].A = T + j * lpad; g[j].lda = ld_t; g[j].M = rows;
-    g[j].W = ls[j]->B; g[j].out = L + static_cast<int64_t>(j) * ls[j]->out; g[j].ldo = ldl;
-    g[j].lora_scale[0] = lora_eff(h, *ls[j]);
+    g[j].W = lora_B(t, lpad); g[j].out = L + static_cast<int64_t>(j) * t.out; g[j].ldo = ldl;
+    g[j].lora_scale[0] = lora_eff(h, t);
     scaled |= g[j].lora_scale[0] != 1.f;
   }
-  return rf::gemm_launch(scaled ? rf::EPI_SCALE : rf::EPI_BIAS, ls[0]->out, lpad, n, g, s);
+  return rf::gemm_launch(scaled ? rf::EPI_SCALE : rf::EPI_BIAS, p.t[0].out, lpad, p.n, g, s);
 }
 
 // The low-rank term of the adaLN Linears added to their sections of `batch` modulation rows:
@@ -459,8 +405,8 @@ int lora_term(rf_dit* h, const LoraT* const* ls, int n, const bf16* A_all, const
 int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bool gated, bool always, bf16* mod, int64_t ld_mod,
                  bf16* tvec, bf16* lvec, cudaStream_t s) {
   const int D = h->D;
-  auto one = [&](const LoraT& t, int64_t off) {
-    return add_vec_lora(h, t, emb, D, batch, 1, mod + off, ld_mod, tvec, lvec, s);
+  auto one = [&](const LoraPack& p, int64_t off) {
+    return add_vec_lora(h, p.t[0], emb, D, batch, 1, mod + off, ld_mod, tvec, lvec, s);
   };
   if (gated) {
     for (int i = 0; i < h->cfg.num_layers; ++i) RF_TRY(one(h->dbl[i].l_norm1, mod_double(h, i, 0, 0)));
@@ -473,287 +419,226 @@ int add_mod_lora(rf_dit* h, const bf16* emb, int batch, bool gated, bool always,
   return 0;
 }
 
-// cond_temb and MODC: step-invariant (transformer.py:108-114 recomputes them every step)
-int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
-  const int D = h->D;
-  // t = c_t * 1000 = 0, guidance = 1000 (s_zero_one = {bf16 0, bf16 1})
-  RF_TRY(compute_temb(h, h->s_zero_one, nullptr, h->s_zero_one + 1, pooled, h->ctemb, s));
-  RF_TRY(rf::gemv_launch(h->ctemb, D, 1, h->modW, h->modB, h->MODC, static_cast<int>(h->n_mod),
-                         static_cast<int>(h->n_mod), D, 1, s));
-  if (!h->any_lora) return 0;
-  // LoRA of norm1.linear / norm.linear acts on silu(cond_temb); tvec [1, lora_pad <= 256] at the front of LT.  (The
-  // condition rows read no norm1_context / norm_out section of MODC.)
-  return add_mod_lora(h, h->ctemb, 1, true, false, h->MODC, h->n_mod, h->LT, h->LT + 256, s);
+// elements of the temb_mod workspace for n vectors
+int64_t temb_ws_elems(const rf_dit* h, int n) {
+  return static_cast<int64_t>(n) * (256 + 9 * h->D + h->lora_pad) + 256 + 3 * h->D;
 }
 
-// fuse_lora mode: merged weights for the condition-token groups (allocated on first use)
-int merge_one(rf_dit* h, const LoraT& t, const bf16* W, bf16** Wm, int rows_off, int out_total,
-              cudaStream_t s) {
-  // target occupies rows [rows_off, rows_off + t.out) of a packed [out_total, t.in] matrix
-  if (*Wm == nullptr) {
-    void* p = nullptr;
-    if (dev_alloc(h, &p, static_cast<size_t>(out_total) * t.in * 2)) return -2;
-    *Wm = static_cast<bf16*>(p);
+// temb_i = time(t_i) + guidance(g) + text(pooled) (CombinedTimestepGuidanceTextProjEmbeddings) for n timesteps, then
+// every adaLN Linear of every block on silu(temb_i) into mod [n, n_mod], with the adaLN LoRA terms of add_mod_lora.
+// The eager step and cond_temb take n = 1; the denoise loop takes every step at once, so the 6.5 GB modulation weight
+// stack is streamed ceil(n/8) times per call instead of once per step.  Same kernels and per-vector arithmetic for
+// any n (the GEMV's per-vector summation order does not depend on the batch width): bit-identical rows.
+int temb_mod(rf_dit* h, int n, const bf16* t, const bf16* guid, const bf16* pooled, bool gated, bool always,
+             bf16* mod, bf16* ws, cudaStream_t s) {
+  const int D = h->D;
+  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c | [n,lora_pad] | [n,6D] (LoRA)
+  bf16* tp = ws;
+  bf16* tmp = tp + static_cast<int64_t>(n) * 256;
+  bf16* a = tmp + static_cast<int64_t>(n) * D;
+  bf16* temb = a + static_cast<int64_t>(n) * D;
+  bf16* gp = temb + static_cast<int64_t>(n) * D;
+  bf16 *tmp1 = gp + 256, *b = tmp1 + D, *c = b + D;
+  bf16* tvec = c + D;                                         // [n, lora_pad]
+  bf16* lvec = tvec + static_cast<int64_t>(n) * h->lora_pad;  // [n, 6D]
+  RF_TRY(rf::timestep_embed_launch(t, nullptr, 1, 1000.0f, tp, n, s));
+  RF_TRY(mlp2(h, tp, 256, n, h->t1, h->l_t1, h->t2, h->l_t2, tmp, a, tvec, lvec, s));
+  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, 1, h->p1, h->l_p1, h->p2, h->l_p2, tmp1, c, tvec, lvec, s));
+  if (h->cfg.guidance_embeds) {
+    RF_TRY(rf::timestep_embed_launch(guid, nullptr, 1, 1000.0f, gp, 1, s));
+    RF_TRY(mlp2(h, gp, 256, 1, h->g1, h->l_g1, h->g2, h->l_g2, tmp1, b, tvec, lvec, s));
   }
-  const size_t off = static_cast<size_t>(rows_off) * t.in;
-  if (!t.set) {  // no adapter on this target: the merged copy is the (possibly reloaded) base weight
-    RF_CHECK_CUDA(cudaMemcpyAsync(*Wm + off, W + off, static_cast<size_t>(t.out) * t.in * 2,
-                                  cudaMemcpyDeviceToDevice, s));
-    return 0;
+  for (int i = 0; i < n; ++i) {
+    bf16* ai = a + static_cast<int64_t>(i) * D;
+    bf16* ti = temb + static_cast<int64_t>(i) * D;
+    if (h->cfg.guidance_embeds) RF_TRY(rf::add3_launch(ai, b, c, ti, D, s));
+    else RF_TRY(rf::add2_launch(ai, c, ti, D, s));
   }
-  return rf::lora_merge_launch(W + off, t.A, t.B, *Wm + off, t.out, t.in, h->lora_pad, lora_eff(h, t), s);
-}
-// an always target (or pack) has a merged copy only once one of its targets is set; until then its groups read the
-// base weight (any_set), so a handle without such adapters allocates nothing here
-bool any_set(const LoraT* const* ls, int n) {
-  for (int k = 0; k < n; ++k)
-    if (ls[k]->set) return true;
-  return false;
-}
-int merge_always(rf_dit* h, const LoraT* const* ls, int n, const bf16* W, bf16** Wm, cudaStream_t s) {
-  if (!any_set(ls, n)) return 0;
-  for (int k = 0; k < n; ++k) RF_TRY(merge_one(h, *ls[k], W, Wm, k * ls[k]->out, n * ls[k]->out, s));
+  RF_TRY(rf::gemv_launch(temb, D, n, h->modW, h->modB, mod, static_cast<int>(h->n_mod), static_cast<int>(h->n_mod),
+                         D, 1, s));
+  if (h->any_lora) RF_TRY(add_mod_lora(h, temb, n, gated, always, mod, h->n_mod, tvec, lvec, s));
   return 0;
 }
+
+// cond_temb and MODC: step-invariant (transformer.py:108-114 recomputes them every step).  t = c_t * 1000 = 0,
+// guidance = 1000 (s_zero_one = {bf16 0, bf16 1}); the condition rows read no norm1_context / norm_out section of MODC.
+int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
+  return temb_mod(h, 1, h->s_zero_one, h->s_zero_one + 1, pooled, true, false, h->MODC, h->emb_ws, s);
+}
+
+// some member of pack p adds a term (lora_on) / is set
+bool pack_on(const rf_dit* h, const LoraPack& p) {
+  for (int k = 0; k < p.n; ++k)
+    if (lora_on(h, p.t[k])) return true;
+  return false;
+}
+bool pack_set(const LoraPack& p) {
+  for (int k = 0; k < p.n; ++k)
+    if (p.t[k].set) return true;
+  return false;
+}
+
+// fuse_lora mode: every projection pack with a target set gets its merged copy (the rows of its unset members are
+// the base weight); the others have none and their groups read the base weight
 int merge_all(rf_dit* h, cudaStream_t s) {
-  const int D = h->D;
-  RF_TRY(merge_one(h, h->l_x_emb, h->x_emb.w, &h->x_emb_m, 0, D, s));
-  const LoraT* lctx = &h->l_ctx;
-  const LoraT* lpo = &h->l_proj_out;
-  RF_TRY(merge_always(h, &lctx, 1, h->ctx_emb.w, &h->ctx_emb_m, s));
-  RF_TRY(merge_always(h, &lpo, 1, h->proj_out.w, &h->proj_out_m, s));
-  for (auto& b : h->dbl) {
-    RF_TRY(merge_one(h, b.l_q, b.qkv.w, &b.qkv_m, 0, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_k, b.qkv.w, &b.qkv_m, D, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_v, b.qkv.w, &b.qkv_m, 2 * D, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_out, b.to_out.w, &b.to_out_m, 0, D, s));
-    RF_TRY(merge_one(h, b.l_ff2, b.ff2.w, &b.ff2_m, 0, D, s));
-    const LoraT* la[3] = {&b.l_aq, &b.l_ak, &b.l_av};
-    const LoraT *lao = &b.l_add_out, *lf1 = &b.l_ff1, *lc1 = &b.l_ffc1, *lc2 = &b.l_ffc2;
-    RF_TRY(merge_always(h, la, 3, b.add_qkv.w, &b.add_qkv_m, s));
-    RF_TRY(merge_always(h, &lao, 1, b.to_add_out.w, &b.to_add_out_m, s));
-    RF_TRY(merge_always(h, &lf1, 1, b.ff1.w, &b.ff1_m, s));
-    RF_TRY(merge_always(h, &lc1, 1, b.ffc1.w, &b.ffc1_m, s));
-    RF_TRY(merge_always(h, &lc2, 1, b.ffc2.w, &b.ffc2_m, s));
-  }
-  for (auto& b : h->sgl) {
-    RF_TRY(merge_one(h, b.l_q, b.qkv.w, &b.qkv_m, 0, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_k, b.qkv.w, &b.qkv_m, D, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_v, b.qkv.w, &b.qkv_m, 2 * D, 3 * D, s));
-    RF_TRY(merge_one(h, b.l_mlp, b.mlp.w, &b.mlp_m, 0, 4 * D, s));
-    RF_TRY(merge_one(h, b.l_out, b.out.w, &b.out_m, 0, D, s));
+  const int lpad = h->lora_pad;
+  for (LoraPack* p : h->proj_packs) {
+    if (!pack_set(*p)) continue;
+    const size_t elems = static_cast<size_t>(p->t[0].out) * p->t[0].in;
+    if (p->Wm == nullptr) {
+      void* q = nullptr;
+      if (dev_alloc(h, &q, p->n * elems * 2)) return -2;
+      p->Wm = static_cast<bf16*>(q);
+    }
+    for (int k = 0; k < p->n; ++k) {
+      const LoraT& t = p->t[k];
+      const size_t off = k * elems;
+      if (t.set)
+        RF_TRY(rf::lora_merge_launch(p->W + off, lora_A(t, lpad), lora_B(t, lpad), p->Wm + off, t.out, t.in, lpad,
+                                     lora_eff(h, t), s));
+      else
+        RF_CHECK_CUDA(cudaMemcpyAsync(p->Wm + off, p->W + off, elems * 2, cudaMemcpyDeviceToDevice, s));
+    }
   }
   h->lora_merged = true;
   h->merged_call_scale = h->call_scale;
   return 0;
 }
 
-// temb_i = time(t_i) + guidance(g) + text(pooled) for ALL steps, then every adaLN Linear of every
-// block for all steps: the 6.5 GB modulation weight stack is streamed ceil(n/8) times per denoise
-// call instead of once per step.  Same kernels, same per-vector arithmetic as compute_temb + gemv
-// (the GEMV's per-vector summation order does not depend on the batch width): bit-identical.
-int precompute_step_mods(rf_dit* h, int n_steps, const bf16* tsteps, const bf16* guid,
-                         const bf16* pooled, cudaStream_t s) {
-  const int D = h->D;
-  // [n,256] | [n,D] tmp | [n,D] a | [n,D] temb | [256] gp | [D] tmp1 | [D] b | [D] c | [n,lora_pad] | [n,6D] (LoRA)
-  bf16* ws = h->s_temb_ws;
-  bf16* tp = ws;
-  bf16* tmp = tp + static_cast<int64_t>(n_steps) * 256;
-  bf16* a = tmp + static_cast<int64_t>(n_steps) * D;
-  bf16* temb = a + static_cast<int64_t>(n_steps) * D;
-  bf16* gp = temb + static_cast<int64_t>(n_steps) * D;
-  bf16 *tmp1 = gp + 256, *b = tmp1 + D, *c = b + D;
-  bf16* tvec = c + D;                                               // [n, lora_pad]
-  bf16* lvec = tvec + static_cast<int64_t>(n_steps) * h->lora_pad;  // [n, 6D]
-  RF_TRY(rf::timestep_embed_launch(tsteps, nullptr, 1, 1000.0f, tp, n_steps, s));
-  // the timestep embedder and its LoRA terms batched over every step, like compute_temb per vector
-  RF_TRY(mlp2(h, tp, 256, n_steps, h->t1, h->l_t1, h->t2, h->l_t2, tmp, a, tvec, lvec, s));
-  RF_TRY(mlp2(h, pooled, h->cfg.pooled_projection_dim, 1, h->p1, h->l_p1, h->p2, h->l_p2, tmp1, c, tvec, lvec, s));
-  if (h->cfg.guidance_embeds) {
-    RF_TRY(rf::timestep_embed_launch(guid, nullptr, 1, 1000.0f, gp, 1, s));
-    RF_TRY(mlp2(h, gp, 256, 1, h->g1, h->l_g1, h->g2, h->l_g2, tmp1, b, tvec, lvec, s));
-  }
-  for (int i = 0; i < n_steps; ++i) {
-    bf16* ai = a + static_cast<int64_t>(i) * D;
-    bf16* ti = temb + static_cast<int64_t>(i) * D;
-    if (h->cfg.guidance_embeds) RF_TRY(rf::add3_launch(ai, b, c, ti, D, s));
-    else RF_TRY(rf::add2_launch(ai, c, ti, D, s));
-  }
-  RF_TRY(rf::gemv_launch(temb, D, n_steps, h->modW, h->modB, h->s_mod_all, static_cast<int>(h->n_mod),
-                         static_cast<int>(h->n_mod), D, 1, s));
-  // the adaLN LoRA terms act on silu(temb_i), which every step knows before the loop: they join the table here too
-  // (latent_lora: the image stream of the double blocks / the txt+img rows of the single blocks; always:
-  // norm1_context and norm_out)
-  if (h->any_lora) RF_TRY(add_mod_lora(h, temb, n_steps, (h->flags & 1) != 0, true, h->s_mod_all, h->n_mod, tvec,
-                                       lvec, s));
-  return 0;
-}
-
+// rows [row0, row0 + rows) of the joint buffers; `cond`: the condition stream
 struct StreamRows {
   int row0, rows;
+  bool cond;
 };
+
+// One projection launch: a group per token stream, each with the adapter pack of the weight it reads
+struct Proj {
+  rf::GemmGroupArgs g[3];
+  StreamRows sr[3];
+  const LoraPack* pack[3];
+  int n = 0;
+  // rows r of out (pitch ldo) = rows r of A (pitch lda) times the Linear w
+  rf::GemmGroupArgs& add(const StreamRows& r, const bf16* A, int lda, const Lin& w, const LoraPack& p, bf16* out,
+                         int ldo) {
+    rf::GemmGroupArgs& a = g[n];
+    memset(&a, 0, sizeof(a));
+    a.A = A + static_cast<int64_t>(r.row0) * lda; a.lda = lda; a.M = r.rows; a.W = w.w; a.bias = w.b;
+    a.out = out + static_cast<int64_t>(r.row0) * ldo; a.ldo = ldo;
+    sr[n] = r;
+    pack[n] = &p;
+    ++n;
+    return a;
+  }
+};
+
+// The rule for which rows carry an adapter: group j of pr carries its pack when the pack is always-on, or the group
+// is the condition stream, or latent_lora is set (lora_controller.py:5-9) - and the pack is on (exact mode) / has a
+// target set (merged mode).  Merged mode points those groups at the merged copy and returns 0.  Exact mode returns
+// the carrying groups in lg, in joint-buffer row order (txt, img / main, cond), which is their order in LT / LL.
+int lora_groups(const rf_dit* h, Proj& pr, int* lg) {
+  int n = 0;
+  for (int j = 0; j < pr.n; ++j) {
+    const LoraPack& p = *pr.pack[j];
+    if (!p.always && !pr.sr[j].cond && !(h->flags & 1)) continue;
+    if (h->use_merged) {
+      if (pack_set(p)) pr.g[j].W = p.Wm;
+    } else if (pack_on(h, p)) {
+      lg[n++] = j;
+    }
+  }
+  std::sort(lg, lg + n, [&](int a, int b) { return pr.sr[a].row0 < pr.sr[b].row0; });
+  return n;
+}
+
+// A projection launch with the LoRA of its carrying groups.  Fast path: T = bf16(x A^T) for all LoRA'd rows in one
+// skinny grouped GEMM (one group per run of rows that are contiguous in the A operand and share their A factor), then
+// ONE grouped launch of all streams in which the eligible groups' tiles carry the low-rank k-block
+// (GemmGroupArgs::lora_T) - L = T B^T never reaches HBM.  Groups too small for it (gemm_lora_eligible) keep the
+// unfused path: L materialised in their rows of LL and added in the epilogue (`addend`); they reuse T when it exists.
+// (t_pre != nullptr: T was already produced by an earlier launch, [rows, ld_t] with this pack's columns at t_pre.)
+int project(rf_dit* h, int epi, int N, int K, Proj& pr, cudaStream_t s, const bf16* t_pre = nullptr, int ld_t = 0) {
+  int lg[3], row[3];
+  const int nl = lora_groups(h, pr, lg);
+  const int lpad = h->lora_pad;
+  bool fused[3] = {false, false, false}, any_fused = false;
+  for (int j = 0, r = 0; j < nl; r += pr.g[lg[j]].M, ++j) {
+    row[j] = r;
+    any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, pr.g[lg[j]]));
+  }
+  if (any_fused && t_pre == nullptr) {
+    ld_t = pr.pack[lg[0]]->n * lpad;
+    rf::GemmGroupArgs dg[3];
+    memset(dg, 0, sizeof(dg));
+    int nd = 0;
+    for (int j = 0; j < nl; ++j) {
+      const rf::GemmGroupArgs& gc = pr.g[lg[j]];
+      const bf16* A = pr.pack[lg[j]]->A;
+      rf::GemmGroupArgs* last = nd ? &dg[nd - 1] : nullptr;
+      if (last && last->W == A && last->lda == gc.lda && gc.A == last->A + static_cast<int64_t>(last->M) * last->lda) {
+        last->M += gc.M;
+        continue;
+      }
+      dg[nd].A = gc.A; dg[nd].lda = gc.lda; dg[nd].M = gc.M; dg[nd].W = A;
+      dg[nd].out = h->LT + static_cast<int64_t>(row[j]) * ld_t; dg[nd].ldo = ld_t;
+      ++nd;
+    }
+    RF_TRY(rf::lora_down_launch(K, ld_t, nd, dg, s));
+    t_pre = h->LT;
+  }
+  for (int j = 0; j < nl; ++j) {
+    const LoraPack& p = *pr.pack[lg[j]];
+    rf::GemmGroupArgs& gc = pr.g[lg[j]];
+    const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(row[j]) * ld_t : nullptr;
+    if (fused[j]) {
+      gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = p.B; gc.lora_sec_cols = p.n > 1 ? p.t[0].out : 0;
+      gc.lora_pad = lpad;
+      for (int k = 0; k < p.n; ++k) gc.lora_scale[k] = lora_eff(h, p.t[k]);
+    } else {
+      bf16* L = h->LL + static_cast<int64_t>(row[j]) * N;
+      RF_TRY(lora_term(h, p, gc.A, gc.lda, gc.M, t_rows, ld_t, L, N, s));
+      gc.addend = L; gc.ldadd = N;
+    }
+  }
+  return rf::gemm_launch(epi, N, K, pr.n, pr.g, s);
+}
 
 // The body of one DiT forward for one sample.  All pointers are device pointers.
 int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16* pooled,
                     const bf16* tstep, const int* step_idx, const bf16* guid, const bf16* cond_lat,
                     bf16* out, cudaStream_t s, const bf16* mod_all = nullptr) {
-  const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D, lpad = h->lora_pad;
+  const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D, C = h->cfg.in_channels, lpad = h->lora_pad;
   const bool use_cond = h->n_cond > 0;
-  // latent_lora (lora_controller.py:5-9): the LoRA also acts on the image stream of the double blocks and on the
-  // txt + img rows of the single blocks (the text stream of the double blocks has no LoRA target)
-  const bool ll = (h->flags & 1) != 0;
-  const StreamRows S_txt{0, h->n_txt}, S_img{h->n_txt, h->n_img}, S_cond{h->n_main, h->n_cond};
+  const StreamRows S_txt{0, h->n_txt, false}, S_img{h->n_txt, h->n_img, false}, S_main{0, h->n_main, false},
+      S_cond{h->n_main, h->n_cond, true};
   bf16 *X = h->X, *XN = h->XN, *QKV = h->QKV, *ACT = h->ACT;
-  auto rowp = [&](bf16* base, int ld, int row) { return base + static_cast<int64_t>(row) * ld; };
-  rf::GemmGroupArgs g[3];
+  // the epilogue operands of a group: RMSNorm weights and RoPE rows (EPI_QKV), gate + residual in place (GATE_RES)
+  auto qk = [&](rf::GemmGroupArgs& a, const StreamRows& r, const bf16* norm_q, const bf16* norm_k) {
+    a.rope_cos = r.cond ? h->crope_cos : h->rope_cos + static_cast<int64_t>(r.row0) * 64;
+    a.rope_sin = r.cond ? h->crope_sin : h->rope_sin + static_cast<int64_t>(r.row0) * 64;
+    a.norm_q = norm_q; a.norm_k = norm_k;
+  };
+  auto gate = [](rf::GemmGroupArgs& a, const bf16* g) {
+    a.res = a.out; a.ldr = a.ldo; a.gate = g;
+  };
 
-  // ---- embedders (transformer.py:91-93,115)
-  memset(g, 0, sizeof(g));
-  g[0].A = latents; g[0].lda = h->cfg.in_channels; g[0].M = h->n_img; g[0].W = h->x_emb.w;
-  g[0].bias = h->x_emb.b; g[0].out = rowp(X, D, S_img.row0); g[0].ldo = D;
-  int ng = 1;
-  if (use_cond) {
-    g[1] = g[0];
-    g[1].A = cond_lat; g[1].M = h->n_cond; g[1].out = rowp(X, D, S_cond.row0);
-    ng = 2;
-  }
-  if (h->use_merged) {
-    if (ll) g[0].W = h->x_emb_m;
-    if (use_cond) g[1].W = h->x_emb_m;
-  } else if (lora_on(h, h->l_x_emb)) {
-    // K = 64, EPI_BIAS: the unfused low-rank term, each LoRA'd group's L in its own rows of LL
-    const LoraT* xl = &h->l_x_emb;
-    int row = 0;
-    for (int j = ll ? 0 : 1; j < ng; ++j) {
-      bf16* L = rowp(h->LL, D, row);
-      RF_TRY(lora_term(h, &xl, 1, xl->A, g[j].A, g[j].lda, g[j].M, nullptr, 0, L, D, s));
-      g[j].addend = L; g[j].ldadd = D;
-      row += g[j].M;
-    }
-  }
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, D, h->cfg.in_channels, ng, g, s));
-  memset(g, 0, sizeof(g));
-  g[0].A = txt; g[0].lda = h->cfg.joint_attention_dim; g[0].M = h->n_txt; g[0].W = h->ctx_emb.w;
-  g[0].bias = h->ctx_emb.b; g[0].out = rowp(X, D, 0); g[0].ldo = D;
-  // context_embedder (always target; EPI_BIAS, K = 4096): the unfused term, like x_embedder's
-  const LoraT* lctx = &h->l_ctx;
-  if (h->use_merged) {
-    if (lctx->set) g[0].W = h->ctx_emb_m;
-  } else if (lora_on(h, *lctx)) {
-    RF_TRY(lora_term(h, &lctx, 1, lctx->A, txt, g[0].lda, g[0].M, nullptr, 0, h->LL, D, s));
-    g[0].addend = h->LL; g[0].ldadd = D;
-  }
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, D, h->cfg.joint_attention_dim, 1, g, s));
+  // ---- embedders (transformer.py:91-93,115); x_embedder reads the latents / condition latents themselves
+  Proj xe;
+  xe.add(S_img, latents, C, h->x_emb, h->l_x_emb, X, D).A = latents;
+  if (use_cond) xe.add(S_cond, cond_lat, C, h->x_emb, h->l_x_emb, X, D).A = cond_lat;
+  RF_TRY(project(h, rf::EPI_BIAS, D, C, xe, s));
+  Proj ce;
+  ce.add(S_txt, txt, h->cfg.joint_attention_dim, h->ctx_emb, h->l_ctx, X, D);
+  RF_TRY(project(h, rf::EPI_BIAS, D, h->cfg.joint_attention_dim, ce, s));
 
   // ---- temb and every modulation vector of the step (transformer.py:95-107 + all adaLN linears)
   if (mod_all != nullptr) {  // denoise loop: this step's row of the precomputed table
     RF_TRY(rf::select_row_launch(mod_all, h->n_mod, step_idx, h->MOD, s));
   } else {
-    RF_TRY(compute_temb(h, tstep, step_idx, guid, pooled, h->temb, s));
-    RF_TRY(rf::gemv_launch(h->temb, D, 1, h->modW, h->modB, h->MOD, static_cast<int>(h->n_mod),
-                           static_cast<int>(h->n_mod), D, 1, s));
-    if (h->any_lora) RF_TRY(add_mod_lora(h, h->temb, 1, ll, true, h->MOD, h->n_mod, h->LT, h->LT + 256, s));
+    RF_TRY(temb_mod(h, 1, tstep, guid, pooled, (h->flags & 1) != 0, true, h->MOD, h->emb_ws, s));
   }
   const bf16* MOD = h->MOD;
   const bf16* MODC = h->MODC;
 
-  auto ln = [&](const StreamRows& sr, const bf16* scale, const bf16* shift) {
-    return rf::ln_modulate_launch(rowp(X, D, sr.row0), D, rowp(XN, D, sr.row0), D, sr.rows, D, scale,
-                                  shift, sr.rows, 0, s);
-  };
-  // The groups of a projection launch that carry the LoRA in exact mode, in row order, each with its target(s) `ls`
-  // and stacked factors A_all / B_all: in the double blocks the text group (its own add_* / to_add_out / ff_context
-  // targets, always on), the image group (under latent_lora; always for ff.net.0.proj), the condition group; in the
-  // single blocks the txt + img group under latent_lora, then the condition group.  `row` is each group's row in
-  // LT / LL: groups are stacked there in this order.
-  struct LoraGrp {
-    int idx, row;
-    const LoraT* const* ls;
-    const bf16 *A_all, *B_all;
-  };
-  struct LoraGroups {
-    int n = 0, rows = 0;
-    LoraGrp e[3];
-    void add(int i, int m, const LoraT* const* ls, const bf16* A_all, const bf16* B_all) {
-      e[n] = LoraGrp{i, rows, ls, A_all, B_all};
-      rows += m;
-      ++n;
-    }
-  };
-  // on: the target(s) of the image (double) / main (single) and condition groups add a term; main_always: the image
-  // group carries it whatever latent_lora says (ff.net.0.proj)
-  auto lora_groups = [&](bool on, int main_idx, int main_rows, int cond_idx, const LoraT* const* ls,
-                         const bf16* A_all, const bf16* B_all, bool main_always = false) {
-    LoraGroups lg;
-    if (!on || h->use_merged) return lg;
-    if (ll || main_always) lg.add(main_idx, main_rows, ls, A_all, B_all);
-    if (use_cond) lg.add(cond_idx, h->n_cond, ls, A_all, B_all);
-    return lg;
-  };
-  // the double blocks: the text group (always targets) first, then the image / condition groups
-  auto lora_groups_dbl = [&](bool txt_on, const LoraT* const* txt_ls, const bf16* txt_A, const bf16* txt_B,
-                             bool on, const LoraT* const* ls, const bf16* A_all, const bf16* B_all,
-                             bool main_always = false) {
-    LoraGroups lg;
-    if (h->use_merged) return lg;
-    if (txt_on) lg.add(1, h->n_txt, txt_ls, txt_A, txt_B);
-    if (on && (ll || main_always)) lg.add(0, h->n_img, ls, A_all, B_all);
-    if (on && use_cond) lg.add(2, h->n_cond, ls, A_all, B_all);
-    return lg;
-  };
-  // merged mode (fuse_lora): the same groups read the merged weights W + B A instead
-  auto merged_w = [&](rf::GemmGroupArgs* gr, int main_idx, int cond_idx, const bf16* Wm, bool main_always = false) {
-    if (!h->use_merged) return;
-    if (ll || main_always) gr[main_idx].W = Wm;
-    if (use_cond) gr[cond_idx].W = Wm;
-  };
-  // A grouped GEMM in which the groups `lg` carry their LoRA (nls = 1 target each, or 3 stacked q|k|v targets).
-  // Fast path: T = bf16(x A^T) for all LoRA'd rows in one skinny grouped GEMM (one group per run of rows that are
-  // contiguous in the A operand and share their A factors), then ONE grouped launch of all streams in which the
-  // eligible groups' tiles carry the low-rank k-block (GemmGroupArgs::lora_T) — L = T B^T never reaches HBM.  Groups
-  // too small for it (gemm_lora_eligible) keep the unfused path: L materialised in their rows of LL and added in the
-  // epilogue (`addend`); they reuse T when it exists.  (t_pre != nullptr: T was already produced by an earlier
-  // launch, [rows, ld_t] with this target's columns at t_pre.)
-  auto gemm_lora = [&](int epi, int N, int K, int ngr, rf::GemmGroupArgs* gr, const LoraGroups& lg, int nls,
-                       int ldl, const bf16* t_pre = nullptr, int ld_t = 0) -> int {
-    bool fused[3] = {false, false, false}, any_fused = false;
-    for (int j = 0; j < lg.n; ++j) any_fused |= (fused[j] = rf::gemm_lora_eligible(epi, N, K, gr[lg.e[j].idx]));
-    if (any_fused && t_pre == nullptr) {
-      ld_t = nls * lpad;
-      rf::GemmGroupArgs dg[3];
-      memset(dg, 0, sizeof(dg));
-      int nd = 0;
-      for (int j = 0; j < lg.n; ++j) {
-        const rf::GemmGroupArgs& gc = gr[lg.e[j].idx];
-        rf::GemmGroupArgs* last = nd ? &dg[nd - 1] : nullptr;
-        if (last && last->W == lg.e[j].A_all && last->lda == gc.lda &&
-            gc.A == last->A + static_cast<int64_t>(last->M) * last->lda) {
-          last->M += gc.M;
-          continue;
-        }
-        dg[nd].A = gc.A; dg[nd].lda = gc.lda; dg[nd].M = gc.M; dg[nd].W = lg.e[j].A_all;
-        dg[nd].out = h->LT + static_cast<int64_t>(lg.e[j].row) * ld_t; dg[nd].ldo = ld_t;
-        ++nd;
-      }
-      RF_TRY(rf::lora_down_launch(K, ld_t, nd, dg, s));
-      t_pre = h->LT;
-    }
-    for (int j = 0; j < lg.n; ++j) {
-      const LoraGrp& e = lg.e[j];
-      rf::GemmGroupArgs& gc = gr[e.idx];
-      const bf16* t_rows = t_pre ? t_pre + static_cast<int64_t>(e.row) * ld_t : nullptr;
-      if (fused[j]) {
-        gc.lora_T = t_rows; gc.ld_t = ld_t; gc.lora_B = e.B_all; gc.lora_sec_cols = nls > 1 ? e.ls[0]->out : 0;
-        gc.lora_pad = lpad;
-        for (int k = 0; k < nls; ++k) gc.lora_scale[k] = lora_eff(h, *e.ls[k]);
-      } else {
-        bf16* L = rowp(h->LL, ldl, e.row);
-        RF_TRY(lora_term(h, e.ls, nls, e.A_all, gc.A, gc.lda, gc.M, t_rows, ld_t, L, ldl, s));
-        gc.addend = L; gc.ldadd = ldl;
-      }
-    }
-    return rf::gemm_launch(epi, N, K, ngr, gr, s);
-  };
   // all token streams of a norm in ONE launch: rows are [txt | img | cond] of the joint buffers
   auto ln3 = [&](const bf16* sc_txt, const bf16* sh_txt, const bf16* sc_img, const bf16* sh_img,
                  const bf16* sc_cond, const bf16* sh_cond) {
@@ -769,6 +654,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
   at.cond_bias = h->attn_cond_bias;
 
   // ================= double-stream blocks (block.py:173-272) =================
+  // groups: img, txt, cond (this order sets the tile schedule); the txt group reads the text stream's own Linears
   for (int i = 0; i < h->cfg.num_layers; ++i) {
     const DoubleBlk& b = h->dbl[i];
     const bf16* mi = MOD + mod_double(h, i, 0, 0);
@@ -778,113 +664,38 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     RF_TRY(ln3(mt + SCALE_MSA * D, mt + SHIFT_MSA * D, mi + SCALE_MSA * D, mi + SHIFT_MSA * D,
                mc + SCALE_MSA * D, mc + SHIFT_MSA * D));
     // q|k|v projections + RMSNorm + RoPE, all streams in one grouped launch
-    memset(g, 0, sizeof(g));
-    g[0].A = rowp(XN, D, S_img.row0); g[0].lda = D; g[0].M = S_img.rows; g[0].W = b.qkv.w;
-    g[0].bias = b.qkv.b; g[0].out = rowp(QKV, D3, S_img.row0); g[0].ldo = D3;
-    g[0].rope_cos = h->rope_cos + static_cast<int64_t>(S_img.row0) * 64;
-    g[0].rope_sin = h->rope_sin + static_cast<int64_t>(S_img.row0) * 64;
-    g[0].norm_q = b.norm_q; g[0].norm_k = b.norm_k;
-    g[1].A = rowp(XN, D, 0); g[1].lda = D; g[1].M = S_txt.rows; g[1].W = b.add_qkv.w;
-    g[1].bias = b.add_qkv.b; g[1].out = rowp(QKV, D3, 0); g[1].ldo = D3;
-    g[1].rope_cos = h->rope_cos; g[1].rope_sin = h->rope_sin;
-    g[1].norm_q = b.norm_added_q; g[1].norm_k = b.norm_added_k;
-    ng = 2;
-    if (use_cond) {
-      g[2] = g[0];
-      g[2].A = rowp(XN, D, S_cond.row0); g[2].M = S_cond.rows;
-      g[2].out = rowp(QKV, D3, S_cond.row0);
-      g[2].rope_cos = h->crope_cos; g[2].rope_sin = h->crope_sin;
-      ng = 3;
-    }
-    merged_w(g, 0, 2, b.qkv_m);
-    const LoraT* dqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    const LoraT* dadd[3] = {&b.l_aq, &b.l_ak, &b.l_av};
-    if (h->use_merged && any_set(dadd, 3)) g[1].W = b.add_qkv_m;
-    LoraGroups lg = lora_groups_dbl(lora_on(h, b.l_aq) || lora_on(h, b.l_ak) || lora_on(h, b.l_av), dadd,
-                                    b.add_qkvA, b.add_qkvB,
-                                    lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), dqkv, b.qkvA,
-                                    b.qkvB);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, 3, D3));
-    else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
+    Proj q;
+    qk(q.add(S_img, XN, D, b.qkv, b.l_qkv, QKV, D3), S_img, b.norm_q, b.norm_k);
+    qk(q.add(S_txt, XN, D, b.add_qkv, b.l_add_qkv, QKV, D3), S_txt, b.norm_added_q, b.norm_added_k);
+    if (use_cond) qk(q.add(S_cond, XN, D, b.qkv, b.l_qkv, QKV, D3), S_cond, b.norm_q, b.norm_k);
+    RF_TRY(project(h, rf::EPI_QKV, D3, D, q, s));
     // joint attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
     RF_TRY(rf::attention_launch(at, s));
     // out projections + gate + residual (in place on X)
-    memset(g, 0, sizeof(g));
-    g[0].A = rowp(ACT, D5, S_img.row0); g[0].lda = D5; g[0].M = S_img.rows; g[0].W = b.to_out.w;
-    g[0].bias = b.to_out.b; g[0].out = rowp(X, D, S_img.row0); g[0].ldo = D;
-    g[0].res = g[0].out; g[0].ldr = D; g[0].gate = mi + GATE_MSA * D;
-    g[1].A = rowp(ACT, D5, 0); g[1].lda = D5; g[1].M = S_txt.rows; g[1].W = b.to_add_out.w;
-    g[1].bias = b.to_add_out.b; g[1].out = rowp(X, D, 0); g[1].ldo = D;
-    g[1].res = g[1].out; g[1].ldr = D; g[1].gate = mt + GATE_MSA * D;
-    ng = 2;
-    if (use_cond) {
-      g[2] = g[0];
-      g[2].A = rowp(ACT, D5, S_cond.row0); g[2].M = S_cond.rows;
-      g[2].out = rowp(X, D, S_cond.row0); g[2].res = g[2].out; g[2].gate = mc + GATE_MSA * D;
-      ng = 3;
-    }
-    merged_w(g, 0, 2, b.to_out_m);
-    const LoraT* dout = &b.l_out;
-    const LoraT* dadd_out = &b.l_add_out;
-    if (h->use_merged && b.l_add_out.set) g[1].W = b.to_add_out_m;
-    lg = lora_groups_dbl(lora_on(h, b.l_add_out), &dadd_out, b.l_add_out.A, b.l_add_out.B, lora_on(h, b.l_out),
-                         &dout, b.l_out.A, b.l_out.B);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D, ng, g, lg, 1, D));
-    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D, ng, g, s));
+    Proj o;
+    gate(o.add(S_img, ACT, D5, b.to_out, b.l_out, X, D), mi + GATE_MSA * D);
+    gate(o.add(S_txt, ACT, D5, b.to_add_out, b.l_add_out, X, D), mt + GATE_MSA * D);
+    if (use_cond) gate(o.add(S_cond, ACT, D5, b.to_out, b.l_out, X, D), mc + GATE_MSA * D);
+    RF_TRY(project(h, rf::EPI_GATE_RES, D, D, o, s));
     // norm2 + modulate
     RF_TRY(ln3(mt + SCALE_MLP * D, mt + SHIFT_MLP * D, mi + SCALE_MLP * D, mi + SHIFT_MLP * D,
                mc + SCALE_MLP * D, mc + SHIFT_MLP * D));
-    // MLP in (GELU-tanh) -> ACT[:, D:5D]
-    memset(g, 0, sizeof(g));
-    g[0].A = rowp(XN, D, S_img.row0); g[0].lda = D; g[0].M = S_img.rows; g[0].W = b.ff1.w;
-    g[0].bias = b.ff1.b; g[0].out = rowp(ACT, D5, S_img.row0) + D; g[0].ldo = D5;
-    g[1] = g[0];
-    g[1].A = rowp(XN, D, 0); g[1].M = S_txt.rows; g[1].W = b.ffc1.w; g[1].bias = b.ffc1.b;
-    g[1].out = rowp(ACT, D5, 0) + D;
-    ng = 2;
-    if (use_cond) {
-      g[2] = g[0];
-      g[2].A = rowp(XN, D, S_cond.row0); g[2].M = S_cond.rows;
-      g[2].out = rowp(ACT, D5, S_cond.row0) + D;
-      ng = 3;
-    }
-    // ff.net.0.proj is inside no enable_lora (block.py:250 names ff.net[2] only): its image rows always carry it
-    if (b.l_ff1.set) merged_w(g, 0, 2, b.ff1_m, true);
-    if (h->use_merged && b.l_ffc1.set) g[1].W = b.ffc1_m;
-    const LoraT* dff1 = &b.l_ff1;
-    const LoraT* dffc1 = &b.l_ffc1;
-    lg = lora_groups_dbl(lora_on(h, b.l_ffc1), &dffc1, b.l_ffc1.A, b.l_ffc1.B, lora_on(h, b.l_ff1), &dff1,
-                         b.l_ff1.A, b.l_ff1.B, true);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, 1, D4));
-    else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
+    // MLP in (GELU-tanh) -> ACT[:, D:5D]; ff.net.0.proj is inside no enable_lora (block.py:250 names ff.net[2] only)
+    Proj f1;
+    f1.add(S_img, XN, D, b.ff1, b.l_ff1, ACT + D, D5);
+    f1.add(S_txt, XN, D, b.ffc1, b.l_ffc1, ACT + D, D5);
+    if (use_cond) f1.add(S_cond, XN, D, b.ff1, b.l_ff1, ACT + D, D5);
+    RF_TRY(project(h, rf::EPI_GELU, D4, D, f1, s));
     // MLP out + gate + residual
-    memset(g, 0, sizeof(g));
-    g[0].A = rowp(ACT, D5, S_img.row0) + D; g[0].lda = D5; g[0].M = S_img.rows; g[0].W = b.ff2.w;
-    g[0].bias = b.ff2.b; g[0].out = rowp(X, D, S_img.row0); g[0].ldo = D;
-    g[0].res = g[0].out; g[0].ldr = D; g[0].gate = mi + GATE_MLP * D;
-    g[1] = g[0];
-    g[1].A = rowp(ACT, D5, 0) + D; g[1].M = S_txt.rows; g[1].W = b.ffc2.w; g[1].bias = b.ffc2.b;
-    g[1].out = rowp(X, D, 0); g[1].res = g[1].out; g[1].gate = mt + GATE_MLP * D;
-    ng = 2;
-    if (use_cond) {
-      g[2] = g[0];
-      g[2].A = rowp(ACT, D5, S_cond.row0) + D; g[2].M = S_cond.rows;
-      g[2].out = rowp(X, D, S_cond.row0); g[2].res = g[2].out; g[2].gate = mc + GATE_MLP * D;
-      ng = 3;
-    }
-    merged_w(g, 0, 2, b.ff2_m);
-    if (h->use_merged && b.l_ffc2.set) g[1].W = b.ffc2_m;
-    const LoraT* dff2 = &b.l_ff2;
-    const LoraT* dffc2 = &b.l_ffc2;
-    lg = lora_groups_dbl(lora_on(h, b.l_ffc2), &dffc2, b.l_ffc2.A, b.l_ffc2.B, lora_on(h, b.l_ff2), &dff2,
-                         b.l_ff2.A, b.l_ff2.B);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D4, ng, g, lg, 1, D));
-    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D4, ng, g, s));
+    Proj f2;
+    gate(f2.add(S_img, ACT + D, D5, b.ff2, b.l_ff2, X, D), mi + GATE_MLP * D);
+    gate(f2.add(S_txt, ACT + D, D5, b.ffc2, b.l_ffc2, X, D), mt + GATE_MLP * D);
+    if (use_cond) gate(f2.add(S_cond, ACT + D, D5, b.ff2, b.l_ff2, X, D), mc + GATE_MLP * D);
+    RF_TRY(project(h, rf::EPI_GATE_RES, D, D4, f2, s));
   }
 
   // ================= single-stream blocks (block.py:275-333) =================
-  const StreamRows S_main{0, h->n_main};
   for (int i = 0; i < h->cfg.num_single_layers; ++i) {
     const SingleBlk& b = h->sgl[i];
     const bf16* mm = MOD + mod_single(h, i, 0);
@@ -892,87 +703,43 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
     // txt and img rows share the block's vectors; the cond rows use the cond_temb ones
     RF_TRY(ln3(mm + 1 * D, mm + 0 * D, mm + 1 * D, mm + 0 * D, mc + 1 * D, mc + 0 * D));
     // q|k|v
-    memset(g, 0, sizeof(g));
-    g[0].A = XN; g[0].lda = D; g[0].M = S_main.rows; g[0].W = b.qkv.w; g[0].bias = b.qkv.b;
-    g[0].out = QKV; g[0].ldo = D3; g[0].rope_cos = h->rope_cos; g[0].rope_sin = h->rope_sin;
-    g[0].norm_q = b.norm_q; g[0].norm_k = b.norm_k;
-    ng = 1;
-    if (use_cond) {
-      g[1] = g[0];
-      g[1].A = rowp(XN, D, S_cond.row0); g[1].M = S_cond.rows;
-      g[1].out = rowp(QKV, D3, S_cond.row0);
-      g[1].rope_cos = h->crope_cos; g[1].rope_sin = h->crope_sin;
-      ng = 2;
-    }
-    merged_w(g, 0, 1, b.qkv_m);
-    const LoraT* sqkv[3] = {&b.l_q, &b.l_k, &b.l_v};
-    LoraGroups lg = lora_groups(lora_on(h, b.l_q) || lora_on(h, b.l_k) || lora_on(h, b.l_v), 0, S_main.rows, 1,
-                                sqkv, b.qkvA, b.qkvB);
+    Proj q;
+    qk(q.add(S_main, XN, D, b.qkv, b.l_qkv, QKV, D3), S_main, b.norm_q, b.norm_k);
+    if (use_cond) qk(q.add(S_cond, XN, D, b.qkv, b.l_qkv, QKV, D3), S_cond, b.norm_q, b.norm_k);
     // exact-mode fast path: T for to_q|to_k|to_v|proj_mlp of all LoRA'd rows in one launch (both GEMMs read the
-    // same XN rows; the q|k|v and the MLP-in launches have the same groups)
-    bool t4 = lg.n > 0 && lora_on(h, b.l_mlp);
-    if (t4) {
-      bool any_fused = false;
-      for (int j = 0; j < lg.n; ++j) any_fused |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, g[lg.e[j].idx]);
-      t4 = any_fused;
+    // same XN rows; the q|k|v and the MLP-in launches have the same LoRA groups)
+    int lg[3], t_rows = 0;
+    const int nl = lora_groups(h, q, lg);
+    bool t4 = false;
+    for (int j = 0; j < nl; ++j) {
+      t4 |= rf::gemm_lora_eligible(rf::EPI_QKV, D3, D, q.g[lg[j]]);
+      t_rows += q.g[lg[j]].M;
     }
-    if (t4)
-      RF_TRY(rf::lora_down_launch(g[lg.e[0].idx].A, D, lg.rows, D, b.qkvA, 4 * lpad, h->LT, 4 * lpad, s));
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_QKV, D3, D, ng, g, lg, 3, D3, t4 ? h->LT : nullptr, 4 * lpad));
-    else RF_TRY(rf::gemm_launch(rf::EPI_QKV, D3, D, ng, g, s));
+    t4 = t4 && pack_on(h, b.l_mlp);
+    if (t4) RF_TRY(rf::lora_down_launch(q.g[lg[0]].A, D, t_rows, D, b.l_qkv.A, 4 * lpad, h->LT, 4 * lpad, s));
+    RF_TRY(project(h, rf::EPI_QKV, D3, D, q, s, t4 ? h->LT : nullptr, 4 * lpad));
     // proj_mlp + GELU -> ACT[:, D:5D]
-    memset(g, 0, sizeof(g));
-    g[0].A = XN; g[0].lda = D; g[0].M = S_main.rows; g[0].W = b.mlp.w; g[0].bias = b.mlp.b;
-    g[0].out = ACT + D; g[0].ldo = D5;
-    ng = 1;
-    if (use_cond) {
-      g[1] = g[0];
-      g[1].A = rowp(XN, D, S_cond.row0); g[1].M = S_cond.rows;
-      g[1].out = rowp(ACT, D5, S_cond.row0) + D;
-      ng = 2;
-    }
-    merged_w(g, 0, 1, b.mlp_m);
-    const LoraT* smlp = &b.l_mlp;
-    lg = lora_groups(lora_on(h, b.l_mlp), 0, S_main.rows, 1, &smlp, b.l_mlp.A, b.l_mlp.B);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GELU, D4, D, ng, g, lg, 1, D4, t4 ? h->LT + 3 * lpad : nullptr, 4 * lpad));
-    else RF_TRY(rf::gemm_launch(rf::EPI_GELU, D4, D, ng, g, s));
+    Proj m;
+    m.add(S_main, XN, D, b.mlp, b.l_mlp, ACT + D, D5);
+    if (use_cond) m.add(S_cond, XN, D, b.mlp, b.l_mlp, ACT + D, D5);
+    RF_TRY(project(h, rf::EPI_GELU, D4, D, m, s, t4 ? h->LT + 3 * lpad : nullptr, 4 * lpad));
     // attention -> ACT[:, 0:D]
     at.out = ACT; at.ldo = D5;
     RF_TRY(rf::attention_launch(at, s));
     // proj_out over cat(attn, mlp) (K = 5D) + gate + residual
-    memset(g, 0, sizeof(g));
-    g[0].A = ACT; g[0].lda = D5; g[0].M = S_main.rows; g[0].W = b.out.w; g[0].bias = b.out.b;
-    g[0].out = X; g[0].ldo = D; g[0].res = X; g[0].ldr = D; g[0].gate = mm + 2 * D;
-    ng = 1;
-    if (use_cond) {
-      g[1] = g[0];
-      g[1].A = rowp(ACT, D5, S_cond.row0); g[1].M = S_cond.rows;
-      g[1].out = rowp(X, D, S_cond.row0); g[1].res = g[1].out; g[1].gate = mc + 2 * D;
-      ng = 2;
-    }
-    merged_w(g, 0, 1, b.out_m);
-    const LoraT* sout = &b.l_out;
-    lg = lora_groups(lora_on(h, b.l_out), 0, S_main.rows, 1, &sout, b.l_out.A, b.l_out.B);
-    if (lg.n) RF_TRY(gemm_lora(rf::EPI_GATE_RES, D, D5, ng, g, lg, 1, D));
-    else RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, D, D5, ng, g, s));
+    Proj o;
+    gate(o.add(S_main, ACT, D5, b.out, b.l_out, X, D), mm + 2 * D);
+    if (use_cond) gate(o.add(S_cond, ACT, D5, b.out, b.l_out, X, D), mc + 2 * D);
+    RF_TRY(project(h, rf::EPI_GATE_RES, D, D5, o, s));
   }
 
   // ================= norm_out + proj_out (transformer.py:241-244) =================
   const bf16* mo = MOD + mod_out(h, 0);  // [scale | shift]
-  RF_TRY(ln(S_img, mo, mo + D));
-  memset(g, 0, sizeof(g));
-  g[0].A = rowp(XN, D, S_img.row0); g[0].lda = D; g[0].M = S_img.rows; g[0].W = h->proj_out.w;
-  g[0].bias = h->proj_out.b; g[0].out = out; g[0].ldo = h->cfg.in_channels;
-  // proj_out (always target; N = 64): the unfused term
-  const LoraT* lpo = &h->l_proj_out;
-  if (h->use_merged) {
-    if (lpo->set) g[0].W = h->proj_out_m;
-  } else if (lora_on(h, *lpo)) {
-    RF_TRY(lora_term(h, &lpo, 1, lpo->A, g[0].A, g[0].lda, g[0].M, nullptr, 0, h->LL, h->cfg.in_channels, s));
-    g[0].addend = h->LL; g[0].ldadd = h->cfg.in_channels;
-  }
-  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, h->cfg.in_channels, D, 1, g, s));
-  return 0;
+  const int64_t img0 = static_cast<int64_t>(S_img.row0) * D;
+  RF_TRY(rf::ln_modulate_launch(X + img0, D, XN + img0, D, S_img.rows, D, mo, mo + D, S_img.rows, 0, s));
+  Proj po;
+  po.add(S_img, XN, D, h->proj_out, h->l_proj_out, out, C).out = out;
+  return project(h, rf::EPI_BIAS, C, D, po, s);
 }
 
 // fuse_lora mode applies when some group carries a LoRA: the condition stream, the image under latent_lora, or the
@@ -986,13 +753,13 @@ bool wants_merged(const rf_dit* h, int n_cond) {
 int lora_rows_needed(const rf_dit* h, int flags, int N, int n_cond) {
   return std::max(((flags & 1) || h->any_always) ? N : n_cond, 1);
 }
-// LT [rows, 4 lora_pad] and LL [rows, 4D], each at least 8D (the adaLN / embedder LoRA scratch)
+// LT [rows, 4 lora_pad] and LL [rows, 4D]
 int alloc_lora_ws(rf_dit* h, int rows) {
-  const size_t r = static_cast<size_t>(rows), least = static_cast<size_t>(8 * h->D) * 2;
+  const size_t r = static_cast<size_t>(rows);
   void* p = nullptr;
-  RF_TRY(dev_alloc(h, &p, std::max(r * 4 * h->lora_pad * 2, least), true));
+  RF_TRY(dev_alloc(h, &p, r * 4 * h->lora_pad * 2, true));
   h->LT = static_cast<bf16*>(p);
-  RF_TRY(dev_alloc(h, &p, std::max(r * 4 * h->D * 2, least), true));
+  RF_TRY(dev_alloc(h, &p, r * 4 * h->D * 2, true));
   h->LL = static_cast<bf16*>(p);
   h->lora_rows = rows;
   return 0;
@@ -1224,16 +991,17 @@ int rf_dit_set_lora(rf_dit* h, const char* module, const void* A, const void* B,
                   " out=" + std::to_string(out_features));
     return -4;
   }
-  RF_TRY(lora_storage(h, t));
-  RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(lpad) * t.in * 2));
-  RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * lpad * 2));
-  RF_CHECK_CUDA(cudaMemcpy(t.A, A, static_cast<size_t>(r) * t.in * 2, cudaMemcpyDeviceToDevice));
-  RF_CHECK_CUDA(cudaMemcpy2D(t.B, lpad * 2, B, static_cast<size_t>(r) * 2,
+  RF_TRY(lora_storage(h, *t.pack));
+  bf16 *tA = lora_A(t, lpad), *tB = lora_B(t, lpad);
+  RF_CHECK_CUDA(cudaMemset(tA, 0, static_cast<size_t>(lpad) * t.in * 2));
+  RF_CHECK_CUDA(cudaMemset(tB, 0, static_cast<size_t>(t.out) * lpad * 2));
+  RF_CHECK_CUDA(cudaMemcpy(tA, A, static_cast<size_t>(r) * t.in * 2, cudaMemcpyDeviceToDevice));
+  RF_CHECK_CUDA(cudaMemcpy2D(tB, lpad * 2, B, static_cast<size_t>(r) * 2,
                              static_cast<size_t>(r) * 2, t.out, cudaMemcpyDeviceToDevice));
   t.set = true;
   t.scale = scale;
   h->any_lora = true;
-  h->any_always |= t.always;
+  h->any_always |= t.pack->always;
   h->lora_merged = false;
   drop_graph(h);  // the captured step may predate this adapter (different launch list)
   return 0;
@@ -1249,8 +1017,8 @@ int rf_dit_clear_lora(rf_dit* h) {
     LoraT& t = *kv.second;
     // zeroed: an unset member of a stacked q|k|v pack still runs in its pack's GEMMs and must add exactly nothing
     if (t.set) {
-      RF_CHECK_CUDA(cudaMemset(t.A, 0, static_cast<size_t>(lpad) * t.in * 2));
-      RF_CHECK_CUDA(cudaMemset(t.B, 0, static_cast<size_t>(t.out) * lpad * 2));
+      RF_CHECK_CUDA(cudaMemset(lora_A(t, lpad), 0, static_cast<size_t>(lpad) * t.in * 2));
+      RF_CHECK_CUDA(cudaMemset(lora_B(t, lpad), 0, static_cast<size_t>(t.out) * lpad * 2));
     }
     t.set = false;
     t.scale = 1.0;
@@ -1352,9 +1120,7 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MOD = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MODC = static_cast<bf16*>(p);
     RF_TRY(alloc_lora_ws(h, lora_rows));
-    if (!(p = A(static_cast<size_t>(512 + 4 * D) * 2))) return -2; h->emb_tmp = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->temb = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(D) * 2))) return -2; h->ctemb = static_cast<bf16*>(p);
+    if (!(p = A(static_cast<size_t>(temb_ws_elems(h, 1)) * 2))) return -2; h->emb_ws = static_cast<bf16*>(p);
     const int C = h->cfg.in_channels;
     if (!(p = A(static_cast<size_t>(batch) * n_img * C * 2))) return -2; h->s_lat = static_cast<bf16*>(p);
     if (!(p = A(static_cast<size_t>(batch) * n_img * C * 2))) return -2; h->s_v = static_cast<bf16*>(p);
@@ -1487,9 +1253,7 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     h->s_sigmas = static_cast<float*>(p);
     if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
     h->s_mod_all = static_cast<bf16*>(p);
-    if (dev_alloc(h, &p, (static_cast<size_t>(n_steps) * (256 + 3 * h->D + h->lora_pad + 6 * h->D) + 256 + 3 * h->D) * 2,
-                  true))
-      return -2;
+    if (dev_alloc(h, &p, static_cast<size_t>(temb_ws_elems(h, n_steps)) * 2, true)) return -2;
     h->s_temb_ws = static_cast<bf16*>(p);
     h->s_cap_steps = n_steps;
     drop_graph(h);  // graph referenced the old arrays
@@ -1520,7 +1284,8 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
           static_cast<size_t>(h->n_cond) * C * 2, cudaMemcpyDeviceToDevice, s));
       RF_TRY(compute_cond_mod(h, h->s_pooled, s));  // hoisted out of the step loop
     }
-    RF_TRY(precompute_step_mods(h, n_steps, h->s_tsteps, h->s_guid, h->s_pooled, s));
+    RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, h->s_pooled, (h->flags & 1) != 0, true, h->s_mod_all,
+                    h->s_temb_ws, s));
     RF_CHECK_CUDA(cudaMemsetAsync(h->s_step, 0, sizeof(int), s));
     // the captured step holds the LoRA scalings as kernel parameters (and skips the terms a zero scaling
     // removes): a changed call scale is re-captured

@@ -114,7 +114,7 @@ class Stream:
 
 def _run_launch(lib, epi, streams, pad, sec_cols, exact, out_pitch=None, out_off=0, heads=None, seed=0,
                 res_pitch=None):
-    """Launch `streams` as one grouped GEMM the way gemm_lora in csrc/dit.cu does (fused LoRA groups of >= 128
+    """Launch `streams` as one grouped GEMM the way project() in csrc/dit.cu does (fused LoRA groups of >= 128
     rows, the unfused EPI_SCALE term into an addend below) and return [(got, ref)] per stream."""
     N, K = streams[0].N, streams[0].K
     nsec = N // sec_cols if sec_cols else 1
@@ -316,7 +316,7 @@ def test_mlp_in_gelu(lib, gemm_path):
 @pytest.mark.parametrize("lpad", [64, 128])
 def test_single_block_shared_T(lib, lpad):
     """T for to_q|to_k|to_v|proj_mlp of all LoRA'd rows in one grouped lora_down (NT = 4 lpad): the txt + img rows
-    contiguous with the shared factors as one group (gemm_lora merges such runs), the cond rows with a second factor
+    contiguous with the shared factors as one group (project() merges such runs), the cond rows with a second factor
     set; then the q|k|v launch reads T at pitch 4 lpad and the GELU launch at column 3 lpad."""
     heads, D = 2, 256
     n_main, n_cond = 640, 192

@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """dev tool: in-process A/B of launch-time switches on the denoise step (entry A 4608 tokens, entry B 5632 tokens
-exact LoRA), alternated in ONE process so that box / clock state is shared.  Switches are environment variables the
-library reads at graph-capture time:  python tools/step_ab.py RF_SIDE_STREAM=1 RF_SIDE_STREAM=0"""
+exact LoRA), alternated in ONE process so that box / clock state is shared.  Each argument is one variant: comma-
+separated KEY=VALUE environment settings applied before its runs, which matter only for a switch the library reads at
+graph-capture time.  The library reads none at present (RF_PDL is read once per process), so without arguments the
+tool times the current build:  python tools/step_ab.py"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
