@@ -74,7 +74,8 @@ int rf_op_linear_lora(int epilogue, int M, int N, int K, const void* x, int ldx,
  * F.scaled_dot_product_attention at train_flux/flux/block.py:123-125 (plus the cat/transpose
  * around it).  cond_mode: 0 = plain; 1 = additive bias `cond_bias` between tokens [0,n_main)
  * and [n_main,n_tok) (attn.c_factor, block.py:115-122); 2 = those cross blocks masked out
- * (union_cond_attn = False, block.py:106-114).  With cond_mode != 0, 0 < n_main < n_tok (any split). */
+ * (union_cond_attn = False, block.py:106-114).  With cond_mode != 0, 0 < n_main < n_tok (any split).
+ * cond_mode 1 with cond_bias = -inf (condition_scale 0: log 0) is computed as cond_mode 2, which it equals. */
 int rf_op_attention(const void* q, const void* k, const void* v, int ld_qkv, void* out, int ld_out,
                     int n_tok, int heads, int batch, int n_main, int cond_mode, float cond_bias,
                     void* stream);

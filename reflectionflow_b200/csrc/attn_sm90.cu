@@ -281,6 +281,9 @@ int attention_launch(const AttnArgs& a, cudaStream_t stream) {
     set_error("attention_launch: output pitch / base must be 4-byte aligned");
     return -1;
   }
+  // cond_bias = -inf (condition_scale 0: the reference's bias log 0) gives the cross pairs a weight of exactly 0, the
+  // cond_mode 2 mask.  Run it as cond_mode 2: a whole cross tile under a -inf tile bias would take -inf - -inf = NaN.
+  const int cond_mode = (a.cond_mode == 1 && a.cond_bias == -INFINITY) ? 2 : a.cond_mode;
   AttnParamsDev p;
   memset(&p, 0, sizeof(p));
   const uint64_t rows = static_cast<uint64_t>(a.n_tok) * a.batch;
@@ -298,8 +301,8 @@ int attention_launch(const AttnArgs& a, cudaStream_t stream) {
   p.batch = a.batch;
   p.q_tiles = (a.n_tok + kTile - 1) / kTile;
   p.kv_tiles = (a.n_tok + kTile - 1) / kTile;
-  p.n_main = a.cond_mode ? a.n_main : a.n_tok;
-  p.cond_mode = a.cond_mode;
+  p.n_main = cond_mode ? a.n_main : a.n_tok;
+  p.cond_mode = cond_mode;
   const float kLog2e = 1.4426950408889634f;
   p.scale_log2 = kLog2e * 0.08838834764831845f;  // 1/sqrt(128)
   p.bias_log2 = kLog2e * a.cond_bias;

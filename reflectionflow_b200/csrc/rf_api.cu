@@ -151,6 +151,23 @@ int rf_dbg_lora_merge(const void* W, const void* A, const void* B, void* Wm, int
                                static_cast<bf16*>(Wm), N, K, R, scale, static_cast<cudaStream_t>(stream));
 }
 
+// the T5 / CLIP attention on the tensor-core path the encoders run (text.cu: small_attn); refuses shapes that path
+// does not take instead of falling back to the CUDA-core kernel
+int rf_dbg_text_attention(const void* q, const void* k, const void* v, int ld, void* out, int ldo, int B, int S,
+                          int heads, const void* bias, float scale, int use_scale, int causal, void* stream) {
+  if (!q || !k || !v || !out || B <= 0 || heads <= 0) {
+    rf::set_error("rf_dbg_text_attention: null operand or empty problem");
+    return -1;
+  }
+  if (!rf::text_attn_tc_eligible(S, ld, ldo)) {
+    rf::set_error("rf_dbg_text_attention: needs 1 <= S <= 512 and 16-byte row pitches");
+    return -1;
+  }
+  return rf::text_attn_tc_launch(static_cast<const bf16*>(q), static_cast<const bf16*>(k), static_cast<const bf16*>(v),
+                                 ld, static_cast<bf16*>(out), ldo, B, S, heads, static_cast<const bf16*>(bias), scale,
+                                 use_scale, causal, static_cast<cudaStream_t>(stream));
+}
+
 
 const char* rf_last_error(void) { return rf::get_error(); }
 int rf_abi_version(void) { return RF_B200_ABI_VERSION; }
