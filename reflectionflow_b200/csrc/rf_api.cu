@@ -168,6 +168,76 @@ int rf_dbg_text_attention(const void* q, const void* k, const void* v, int ld, v
                                  use_scale, causal, static_cast<cudaStream_t>(stream));
 }
 
+// Test hooks over the VAE's launchers (csrc/vae.cu, the convolution in csrc/gemm_sm90.cu): the same host code
+// rf_vae_decode / rf_vae_encode run, on caller-owned buffers.  Layouts: rf_internal.h.
+int rf_dbg_vae_conv(const void* in, const void* weight, const void* bias, void* out, const void* res, const void* ones,
+                    int H, int W, int Cin, int Cout, int taps, int stride, void* stream) {
+  return rf::conv_launch(static_cast<const bf16*>(in), static_cast<const bf16*>(weight), static_cast<const bf16*>(bias),
+                         static_cast<bf16*>(out), static_cast<const bf16*>(res), static_cast<const bf16*>(ones), H, W,
+                         Cin, Cout, taps, stride, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_conv_repack(const void* src, void* dst, int Cout, int Cin, int taps, int Cout_pad, int Cin_pad,
+                           void* stream) {
+  return rf::conv_repack_launch(static_cast<const bf16*>(src), static_cast<bf16*>(dst), Cout, Cin, taps, Cout_pad,
+                                Cin_pad, static_cast<cudaStream_t>(stream));
+}
+
+// part: rf_dbg_vae_gn_part_floats() floats; mean_rstd: 64 floats (the 32 group means, then the 32 values of 1 / std)
+int rf_dbg_vae_gn_part_floats(void) { return rf::gn_part_floats; }
+int rf_dbg_vae_group_norm(const void* x, void* out, int H, int W, int C, const void* gamma, const void* beta, int silu,
+                          int in_padded, int out_padded, float* part, float* mean_rstd, void* stream) {
+  return rf::group_norm_launch(static_cast<const bf16*>(x), static_cast<bf16*>(out), H, W, C,
+                               static_cast<const bf16*>(gamma), static_cast<const bf16*>(beta), silu, in_padded,
+                               out_padded, part, mean_rstd, static_cast<cudaStream_t>(stream));
+}
+
+// the mid-block attention of a loaded rf_vae handle (encoder 0: decoder.mid_block, 1: encoder.mid_block)
+int rf_dbg_vae_mid_attention(rf_vae* h, int encoder, const void* x, void* out, int H, int W, void* stream) {
+  return vae_mid_attention(h, encoder, static_cast<const bf16*>(x), static_cast<bf16*>(out), H, W,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_softmax_rows(void* s, int rows, int n, int valid, float scale, void* stream) {
+  return rf::softmax_rows_launch(static_cast<bf16*>(s), rows, n, valid, scale, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_unpack_latents(const void* packed, void* out, int h, int w, float scaling, float shift, void* stream) {
+  return rf::unpack_latents_launch(static_cast<const bf16*>(packed), static_cast<bf16*>(out), h, w, scaling, shift,
+                                   static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_upsample2x(const void* x, void* out, int H, int W, int C, void* stream) {
+  return rf::upsample2x_launch(static_cast<const bf16*>(x), static_cast<bf16*>(out), H, W, C,
+                               static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_repad(const void* x, void* out, int H, int W, int C, int in_padded, int out_padded, void* stream) {
+  return rf::repad_launch(static_cast<const bf16*>(x), static_cast<bf16*>(out), H, W, C, in_padded, out_padded,
+                          static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_transpose(const void* in, int ld_in, void* out, int rows, int cols, void* stream) {
+  return rf::transpose_launch(static_cast<const bf16*>(in), ld_in, static_cast<bf16*>(out), rows, cols,
+                              static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_postprocess(const void* x, int H, int W, int C, uint8_t* u8, void* chw, void* stream) {
+  return rf::postprocess_launch(static_cast<const bf16*>(x), H, W, C, u8, static_cast<bf16*>(chw),
+                                static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_image_to_nhwc(const uint8_t* u8, const void* chw, void* out, int H, int W, void* stream) {
+  return rf::image_to_nhwc_launch(u8, static_cast<const bf16*>(chw), static_cast<bf16*>(out), H, W,
+                                  static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_vae_sample_pack(const void* mom, int C, const void* eps, void* packed, int h, int w, float scaling,
+                           float shift, void* stream) {
+  return rf::sample_pack_launch(static_cast<const bf16*>(mom), C, static_cast<const bf16*>(eps),
+                                static_cast<bf16*>(packed), h, w, scaling, shift, static_cast<cudaStream_t>(stream));
+}
+
 
 const char* rf_last_error(void) { return rf::get_error(); }
 int rf_abi_version(void) { return RF_B200_ABI_VERSION; }

@@ -175,4 +175,48 @@ int add_rows_launch(bf16* dst, int64_t ldd, const bf16* src, int lds, int rows, 
 int lora_merge_launch(const bf16* W, const bf16* A, const bf16* B, bf16* Wm, int N, int K, int R, float scale,
                       cudaStream_t stream);
 
+// ---------------------------------------------------------------------------- VAE (vae.cu, conv: gemm_sm90.cu)
+// Images are NHWC bf16; "padded" means a one-pixel zero ring: [(H+2)(W+2), C].  Every writer below stores interior
+// pixels only and leaves the ring as it found it.
+//
+// 3x3 (taps = 9) or 1x1 (taps = 1) convolution, stride 1 (zero padding 1) or stride 2 (diffusers Downsample2D: pad
+// right / bottom by one), padded in [(Hin+2)(Win+2), Cin] -> padded out [(H+2)(W+2), Cout] (H, W: output size, Hin =
+// stride H), weight [Cout, taps * Cin] tap-major (conv_repack_launch), out = bf16(acc + bias) or, with res (same
+// geometry as out, may alias it), bf16(res + bf16(ones * bf16(acc + bias))).  Cin % 64 == 0, Cout % 128 == 0.
+int conv_launch(const bf16* in, const bf16* weight, const bf16* bias, bf16* out, const bf16* res,
+                const bf16* ones, int H, int W, int Cin, int Cout, int taps, int stride, cudaStream_t stream);
+// torch conv weight [Cout, Cin, kh, kw] -> [Cout_pad, taps * Cin_pad], tap-major K, zero padded
+int conv_repack_launch(const bf16* src, bf16* dst, int Cout, int Cin, int taps, int Cout_pad, int Cin_pad,
+                       cudaStream_t stream);
+// GroupNorm(32, eps 1e-6) [+ SiLU] of a padded H x W x C image (C = 128, 256 or 512) into a padded or compact one.
+// part: gn_part_floats floats of block partials; mean_rstd: 64 floats, [0, 32) the group means, [32, 64) 1 / std.
+constexpr int kGnBlocks = 132 * 4;
+constexpr int gn_part_floats = 2 * 128 * kGnBlocks;
+int group_norm_launch(const bf16* x, bf16* out, int H, int W, int C, const bf16* gamma, const bf16* beta, int silu,
+                      int in_padded, int out_padded, float* part, float* mean_rstd, cudaStream_t stream);
+// packed latents [(h/2)(w/2), 64] -> bf16(bf16(z / scaling) + shift) into channels 0..15 of padded [.., 64]
+int unpack_latents_launch(const bf16* packed, bf16* out, int h, int w, float scaling, float shift,
+                          cudaStream_t stream);
+// nearest 2x: padded [(H+2)(W+2), C] -> padded [(2H+2)(2W+2), C]
+int upsample2x_launch(const bf16* x, bf16* out, int H, int W, int C, cudaStream_t stream);
+// padded <-> compact [H W, C] row copies
+int repad_launch(const bf16* x, bf16* out, int H, int W, int C, int in_padded, int out_padded, cudaStream_t stream);
+// in place, each of `rows` rows of n bf16 scores (n % 8 == 0): softmax(s * scale) over keys [0, valid), 0 after
+int softmax_rows_launch(bf16* s, int rows, int n, int valid, float scale, cudaStream_t stream);
+// out[c, r] = in[r, c] for r < rows, c < cols (both multiples of 32); out pitch rows
+int transpose_launch(const bf16* in, int ld_in, bf16* out, int rows, int cols, cudaStream_t stream);
+// channels 0..2 of padded [.., C] -> uint8 HWC (VaeImageProcessor.postprocess) and / or bf16 CHW
+int postprocess_launch(const bf16* x, int H, int W, int C, uint8_t* u8, bf16* chw, cudaStream_t stream);
+// uint8 HWC (u8 / 255 * 2 - 1 in fp32, then bf16) or bf16 CHW -> channels 0..2 of padded [.., 64]
+int image_to_nhwc_launch(const uint8_t* u8, const bf16* chw, bf16* out, int H, int W, cudaStream_t stream);
+// moments (padded [.., C]: mean 0..15, logvar 16..31) -> posterior sample (eps bf16 [16, h, w] or NULL = mode)
+// -> bf16((z - shift) * scaling) -> packed [(h/2)(w/2), 64]
+int sample_pack_launch(const bf16* mom, int C, const bf16* eps, bf16* packed, int h, int w, float scaling,
+                       float shift, cudaStream_t stream);
+
 }  // namespace rf
+
+// The mid-block self-attention of a loaded VAE (encoder = 0: the decoder's, 1: the encoder's) at latent H x W:
+// GroupNorm -> to_q | to_k | to_v -> softmax(q k^T / sqrt(512)) v -> to_out + x, padded [.., 512] in and out.
+struct rf_vae;
+int vae_mid_attention(rf_vae* h, int encoder, const rf::bf16* x, rf::bf16* out, int H, int W, cudaStream_t stream);

@@ -21,9 +21,6 @@
 #include "rf_ptx.cuh"
 
 namespace rf {
-int conv_launch(const bf16* in, const bf16* weight, const bf16* bias, bf16* out, const bf16* res,
-                const bf16* ones, int H, int W, int Cin, int Cout, int taps, int stride,
-                cudaStream_t stream);
 
 // ------------------------------------------------------------------ weight repack
 // torch conv weight [Cout, Cin, kh, kw] -> [Cout_pad, (kh*kw) * Cin_pad], tap-major K, zero padded
@@ -61,7 +58,9 @@ __global__ void unpack_latents_kernel(const bf16* __restrict__ packed, bf16* __r
 // Deterministic (no atomics): fixed-order reduction inside the block, one partial row per block,
 // partial rows summed in block order by the finalize kernel — a run-to-run difference in the last
 // bit of a mean could flip a bf16 rounding downstream and with it a candidate's score.
-static constexpr int kGnBlocks = 132 * 4;
+// The sums are of x - p, p = the group's first channel at the first interior pixel: E[x^2] - E[x]^2 from fp32 sums
+// of x itself loses (mean / std)^2 of the variance's bits (2.9e-3 relative error of 1 / std at mean / std = 128 and
+// 1024^2 pixels); shifted by a sample of the group, the sums hold the spread around that sample instead.
 __global__ void __launch_bounds__(256)
 gn_stats_kernel(const bf16* __restrict__ x, int H, int W, int C, int padded, float* __restrict__ part) {
   __shared__ float sm[256][4];
@@ -72,16 +71,22 @@ gn_stats_kernel(const bf16* __restrict__ x, int H, int W, int C, int padded, flo
   const int wshift = (W & (W - 1)) == 0 ? __ffs(W) - 1 : -1;
   float s0 = 0.f, q0 = 0.f, s1 = 0.f, q1 = 0.f;
   if (my_p < pix_per_iter) {
+    const int cpg = C / 32;
+    const bf16* first = x + (padded ? static_cast<size_t>(W + 3) : 0) * C;
+    const float p0 = __bfloat162float(first[(my_oct * 8) / cpg * cpg]);
+    const float p1 = __bfloat162float(first[(my_oct * 8 + 4) / cpg * cpg]);
     for (int p = blockIdx.x * pix_per_iter + my_p; p < npix; p += gridDim.x * pix_per_iter) {
       const int y = wshift >= 0 ? (p >> wshift) : (p / W), xx = p - y * W;
       const size_t row = padded ? static_cast<size_t>(y + 1) * (W + 2) + xx + 1 : static_cast<size_t>(p);
       const uint4 u = __ldg(reinterpret_cast<const uint4*>(x + row * C) + my_oct);
       const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z),
                    d = unpack_bf16x2(u.w);
-      s0 += a.x + a.y + b.x + b.y;
-      q0 += a.x * a.x + a.y * a.y + b.x * b.x + b.y * b.y;
-      s1 += c.x + c.y + d.x + d.y;
-      q1 += c.x * c.x + c.y * c.y + d.x * d.x + d.y * d.y;
+      const float a0 = a.x - p0, a1 = a.y - p0, b0 = b.x - p0, b1 = b.y - p0;
+      const float c0 = c.x - p1, c1 = c.y - p1, d0 = d.x - p1, d1 = d.y - p1;
+      s0 += a0 + a1 + b0 + b1;
+      q0 += a0 * a0 + a1 * a1 + b0 * b0 + b1 * b1;
+      s1 += c0 + c1 + d0 + d1;
+      q1 += c0 * c0 + c1 * c1 + d0 * d0 + d1 * d1;
     }
   }
   sm[threadIdx.x][0] = s0; sm[threadIdx.x][1] = q0; sm[threadIdx.x][2] = s1; sm[threadIdx.x][3] = q1;
@@ -99,9 +104,10 @@ gn_stats_kernel(const bf16* __restrict__ x, int H, int W, int C, int padded, flo
 }
 // one warp per group: lane l sums partials l, l + 32, ... in double, then a fixed shuffle tree (deterministic).
 // (One thread per group walked 592 x C/128 dependent loads: 10-45 us per norm, 30 norms per decode.)
+// The partials are sums of x - p (gn_stats_kernel); the finalize reads the same p and adds it back to the mean.
 __global__ void __launch_bounds__(1024)
-gn_finalize_kernel(const float* __restrict__ part, int nblocks, int C, double count,
-                   float* __restrict__ mean_rstd) {
+gn_finalize_kernel(const float* __restrict__ part, int nblocks, int C, double count, const bf16* __restrict__ x,
+                   int W, int padded, float* __restrict__ mean_rstd) {
   const int g = threadIdx.x >> 5, lane = threadIdx.x & 31;  // 32 groups
   const int nsub = C >> 2, per = nsub / 32;
   double s = 0, q = 0;
@@ -116,11 +122,12 @@ gn_finalize_kernel(const float* __restrict__ part, int nblocks, int C, double co
     q += __shfl_xor_sync(0xffffffffu, q, o);
   }
   if (lane == 0) {
+    const double pivot = __bfloat162float(x[(padded ? static_cast<size_t>(W + 3) : 0) * C + g * (C / 32)]);
     const double n = count * (C / 32);
-    const double mean = s / n;
-    double var = q / n - mean * mean;
+    const double d = s / n;
+    double var = q / n - d * d;
     if (var < 0) var = 0;
-    mean_rstd[g] = static_cast<float>(mean);
+    mean_rstd[g] = static_cast<float>(pivot + d);
     mean_rstd[32 + g] = static_cast<float>(1.0 / sqrt(var + 1e-6));
   }
 }
@@ -343,6 +350,117 @@ __global__ void sample_pack_kernel(const bf16* __restrict__ mom, int C, const bf
   packed[static_cast<size_t>(tok) * 64 + ch] = __float2bfloat16_rn(z);
 }
 
+// ------------------------------------------------------------------ launchers (rf_internal.h)
+static int grid_for(long long work, int threads = 256) {
+  long long b = (work + threads - 1) / threads;
+  if (b > 132 * 16) b = 132 * 16;
+  return static_cast<int>(b < 1 ? 1 : b);
+}
+
+int conv_repack_launch(const bf16* src, bf16* dst, int Cout, int Cin, int taps, int Cout_pad, int Cin_pad,
+                       cudaStream_t stream) {
+  const long long total = static_cast<long long>(Cout_pad) * taps * Cin_pad;
+  repack_conv_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, stream>>>(src, dst, Cout, Cin, taps, Cin_pad,
+                                                                                total);
+  RF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int group_norm_launch(const bf16* x, bf16* out, int H, int W, int C, const bf16* gamma, const bf16* beta, int silu,
+                      int in_padded, int out_padded, float* part, float* mean_rstd, cudaStream_t s) {
+  if (C % 128 != 0 || 256 % (C / 8) != 0) {
+    set_error("group_norm: channels must be 128, 256 or 512");
+    return -1;
+  }
+  {
+    ProfScope prof("vae_gn_stats", 0, 2.0 * H * W * C, s);
+    gn_stats_kernel<<<kGnBlocks, 256, 0, s>>>(x, H, W, C, in_padded, part);
+  }
+  RF_CHECK_CUDA(cudaGetLastError());
+  gn_finalize_kernel<<<1, 1024, 0, s>>>(part, kGnBlocks, C, static_cast<double>(H) * W, x, W, in_padded, mean_rstd);
+  {
+    ProfScope prof("vae_gn_apply", 0, 4.0 * H * W * C, s);
+    // rows x row slices: ~16 CTAs per SM in flight, every thread >= 1 vector of its row slice
+    const int rows = H < 132 * 16 ? H : 132 * 16;
+    int slices = (132 * 16 + rows - 1) / rows;
+    const int max_slices = (W * (C / 8) + 255) / 256;
+    if (slices > max_slices) slices = max_slices;
+    gn_apply_kernel<<<dim3(rows, slices), 256, 0, s>>>(x, out, H, W, C, mean_rstd, gamma, beta, silu, in_padded,
+                                                      out_padded);
+  }
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch(3);
+  return 0;
+}
+
+int unpack_latents_launch(const bf16* packed, bf16* out, int h, int w, float scaling, float shift,
+                          cudaStream_t s) {
+  unpack_latents_kernel<<<(h * w * 16 + 255) / 256, 256, 0, s>>>(packed, out, h, w, scaling, shift);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int upsample2x_launch(const bf16* x, bf16* out, int H, int W, int C, cudaStream_t s) {
+  {
+    ProfScope prof("vae_upsample", 0, 10.0 * H * W * C, s);
+    upsample2x_kernel<<<grid_for(static_cast<long long>(4) * H * W * (C / 8)), 256, 0, s>>>(x, out, H, W, C);
+  }
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int repad_launch(const bf16* x, bf16* out, int H, int W, int C, int in_padded, int out_padded, cudaStream_t s) {
+  repad_kernel<<<grid_for(static_cast<long long>(H) * W * (C / 8)), 256, 0, s>>>(x, out, H, W, C, in_padded,
+                                                                                out_padded);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int softmax_rows_launch(bf16* S, int rows, int n, int valid, float scale, cudaStream_t s) {
+  {
+    ProfScope prof("vae_softmax", 0, 4.0 * rows * n, s);
+    softmax_rows_kernel<<<rows, 256, 0, s>>>(S, n, valid, scale);
+  }
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int transpose_launch(const bf16* in, int ld_in, bf16* out, int rows, int cols, cudaStream_t s) {
+  dim3 tg(cols / 32, rows / 32), tb(32, 8);
+  transpose_kernel<<<tg, tb, 0, s>>>(in, ld_in, out, rows, cols);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int postprocess_launch(const bf16* x, int H, int W, int C, uint8_t* u8, bf16* chw, cudaStream_t s) {
+  postprocess_kernel<<<static_cast<int>((static_cast<long long>(H) * W + 255) / 256), 256, 0, s>>>(x, H, W, C, u8,
+                                                                                                 chw);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int image_to_nhwc_launch(const uint8_t* u8, const bf16* chw, bf16* out, int H, int W, cudaStream_t s) {
+  image_to_nhwc_kernel<<<static_cast<int>((static_cast<long long>(H) * W + 255) / 256), 256, 0, s>>>(u8, chw, out,
+                                                                                                   H, W);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int sample_pack_launch(const bf16* mom, int C, const bf16* eps, bf16* packed, int h, int w, float scaling,
+                       float shift, cudaStream_t s) {
+  sample_pack_kernel<<<(h * w * 16 + 255) / 256, 256, 0, s>>>(mom, C, eps, packed, h, w, scaling, shift);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
 }  // namespace rf
 
 using rf::bf16;
@@ -492,38 +610,9 @@ size_t padded_elems(int H, int W, int C) { return static_cast<size_t>(H + 2) * (
 // keys of the mid-block attention, padded to whole 128-row tiles (the S GEMM's N, the PV GEMM's K)
 int padded_tokens(int H, int W) { return (H * W + 127) / 128 * 128; }
 
-int grid_for(long long work, int threads = 256) {
-  long long b = (work + threads - 1) / threads;
-  if (b > 132 * 16) b = 132 * 16;
-  return static_cast<int>(b < 1 ? 1 : b);
-}
-
 int group_norm(rf_vae* h, const bf16* x, bf16* out, int H, int W, const Norm& n, int silu,
                int in_padded, int out_padded, cudaStream_t s) {
-  const int C = n.c;
-  if (C % 128 != 0 || 256 % (C / 8) != 0) {
-    rf::set_error("group_norm: channels must be 128, 256 or 512");
-    return -1;
-  }
-  {
-    rf::ProfScope prof("vae_gn_stats", 0, 2.0 * H * W * C, s);
-    rf::gn_stats_kernel<<<rf::kGnBlocks, 256, 0, s>>>(x, H, W, C, in_padded, h->gn_acc);
-  }
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::gn_finalize_kernel<<<1, 1024, 0, s>>>(h->gn_acc, rf::kGnBlocks, C, static_cast<double>(H) * W, h->gn_mr);
-  {
-    rf::ProfScope prof("vae_gn_apply", 0, 4.0 * H * W * C, s);
-    // rows x row slices: ~16 CTAs per SM in flight, every thread >= 1 vector of its row slice
-    const int rows = H < 132 * 16 ? H : 132 * 16;
-    int slices = (132 * 16 + rows - 1) / rows;
-    const int max_slices = (W * (C / 8) + 255) / 256;
-    if (slices > max_slices) slices = max_slices;
-    rf::gn_apply_kernel<<<dim3(rows, slices), 256, 0, s>>>(
-        x, out, H, W, C, h->gn_mr, n.g, n.b, silu, in_padded, out_padded);
-  }
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch(3);
-  return 0;
+  return rf::group_norm_launch(x, out, H, W, n.c, n.g, n.b, silu, in_padded, out_padded, h->gn_acc, h->gn_mr, s);
 }
 int conv(rf_vae* h, const ConvW& c, const bf16* in, bf16* out, const bf16* res, int H, int W,
          cudaStream_t s) {
@@ -595,7 +684,7 @@ int ensure_workspace(rf_vae* h, int H, int W) {  // H, W: output image size
   RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->ao = static_cast<bf16*>(p);
   RF_TRYV(valloc(h, &p, npad * 512 * 2)); h->ay = static_cast<bf16*>(p);
   if (!h->gn_acc) {
-    RF_TRYV(valloc(h, &p, sizeof(float) * 2 * 128 * rf::kGnBlocks)); h->gn_acc = static_cast<float*>(p);
+    RF_TRYV(valloc(h, &p, sizeof(float) * rf::gn_part_floats)); h->gn_acc = static_cast<float*>(p);
     RF_TRYV(valloc(h, &p, sizeof(float) * 64)); h->gn_mr = static_cast<float*>(p);
   }
   h->ws_h = H; h->ws_w = W;
@@ -630,18 +719,14 @@ int resnet(rf_vae* h, const Resnet& r, int x, int out, int t1, int t2, int H, in
   return conv(h, r.c2, h->buf[t1], h->buf[out], shortcut, H, W, s);
 }
 
-// UNetMidBlock2D: resnet, self-attention over H*W tokens (1 head x 512), resnet.  buf[x] -> buf[x].
+// The mid-block's self-attention over H*W tokens (1 head x 512): x (padded) -> out (padded, interior only).
 // The keys run to npad = padded_tokens(H, W): K / V rows [ntok, npad) are zero and the softmax gives them
 // probability 0, so the padding changes no result.  With ntok % 128 == 0 there is no padding.
-int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int H, int W, cudaStream_t s) {
-  RF_TRYV(resnet(h, m.res[0], x, y, t1, t2, H, W, s));
-  std::swap(x, y);
+int mid_attention(rf_vae* h, const MidBlock& m, const bf16* x, bf16* out, int H, int W, cudaStream_t s) {
   const int ntok = H * W, npad = padded_tokens(H, W);
-  RF_TRYV(group_norm(h, h->buf[x], h->tok, H, W, m.attn_gn, 0, 1, 0, s));  // compact tokens
-  rf::repad_kernel<<<grid_for(static_cast<long long>(ntok) * 64), 256, 0, s>>>(h->buf[x], h->tokx, H, W, 512,
-                                                                              1, 0);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYV(rf::group_norm_launch(x, h->tok, H, W, 512, m.attn_gn.g, m.attn_gn.b, 0, 1, 0, h->gn_acc, h->gn_mr,
+                                s));  // compact tokens
+  RF_TRYV(rf::repad_launch(x, h->tokx, H, W, 512, 1, 0, s));
   rf::GemmGroupArgs g;
   memset(&g, 0, sizeof(g));  // q | k | v
   g.A = h->tok; g.lda = 512; g.M = ntok; g.W = m.attn_qkv.w; g.bias = m.attn_qkv.b;
@@ -657,16 +742,8 @@ int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int 
   memset(&g, 0, sizeof(g));  // S = Q K^T  [ntok, npad]
   g.A = h->qkv; g.lda = 1536; g.M = ntok; g.W = h->ay; g.out = h->S; g.ldo = npad;
   RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, npad, 512, 1, &g, s));
-  {
-    rf::ProfScope prof("vae_softmax", 0, 4.0 * ntok * npad, s);
-    rf::softmax_rows_kernel<<<ntok, 256, 0, s>>>(h->S, npad, ntok, 1.0f / sqrtf(512.0f));
-  }
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
-  dim3 tg(512 / 32, npad / 32), tb(32, 8);
-  rf::transpose_kernel<<<tg, tb, 0, s>>>(h->qkv + 1024, 1536, h->vt, npad, 512);  // V^T [512, npad]
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYV(rf::softmax_rows_launch(h->S, ntok, npad, ntok, 1.0f / sqrtf(512.0f), s));
+  RF_TRYV(rf::transpose_launch(h->qkv + 1024, 1536, h->vt, npad, 512, s));  // V^T [512, npad]
   memset(&g, 0, sizeof(g));  // O = P V
   g.A = h->S; g.lda = npad; g.M = ntok; g.W = h->vt; g.out = h->ao; g.ldo = 512;
   RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 512, npad, 1, &g, s));
@@ -674,11 +751,15 @@ int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int 
   g.A = h->ao; g.lda = 512; g.M = ntok; g.W = m.attn_out.w; g.bias = m.attn_out.b;
   g.out = h->ay; g.ldo = 512; g.res = h->tokx; g.ldr = 512; g.gate = h->ones;
   RF_TRYV(rf::gemm_launch(rf::EPI_GATE_RES, 512, 512, 1, &g, s));
+  return rf::repad_launch(h->ay, out, H, W, 512, 0, 1, s);
+}
+
+// UNetMidBlock2D: resnet, self-attention, resnet.  buf[x] -> buf[x].
+int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int H, int W, cudaStream_t s) {
+  RF_TRYV(resnet(h, m.res[0], x, y, t1, t2, H, W, s));
+  std::swap(x, y);
   RF_TRYV(prep(h, y, H, W, 512, s));
-  rf::repad_kernel<<<grid_for(static_cast<long long>(ntok) * 64), 256, 0, s>>>(h->ay, h->buf[y], H, W, 512,
-                                                                              0, 1);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYV(mid_attention(h, m, h->buf[x], h->buf[y], H, W, s));
   std::swap(x, y);
   RF_TRYV(resnet(h, m.res[1], x, y, t1, t2, H, W, s));
   std::swap(x, y);
@@ -867,10 +948,7 @@ int rf_vae_load_weight(rf_vae* h, const char* key, const void* src, int64_t nume
   if (sl.kind == 0) {
     ConvW& c = *static_cast<ConvW*>(sl.obj);
     if (numel != static_cast<int64_t>(c.cout) * c.cin * c.taps) return bad(static_cast<int64_t>(c.cout) * c.cin * c.taps);
-    const long long total = static_cast<long long>(c.cout_pad) * c.taps * c.cin_pad;
-    rf::repack_conv_kernel<<<static_cast<int>((total + 255) / 256), 256>>>(s, c.w, c.cout, c.cin, c.taps,
-                                                                          c.cin_pad, total);
-    RF_CHECK_CUDA(cudaGetLastError());
+    RF_TRYV(rf::conv_repack_launch(s, c.w, c.cout, c.cin, c.taps, c.cout_pad, c.cin_pad, nullptr));
     c.w_loaded = true;
   } else if (sl.kind == 1) {
     ConvW& c = *static_cast<ConvW*>(sl.obj);
@@ -935,10 +1013,8 @@ static int decode_body(rf_vae* h, const void* packed_latents, int height, int wi
   const int t1 = 2, t2 = 3;
   // ---- latents -> NHWC (16 real channels of 64), conv_in
   RF_TRYV(prep(h, x, H, W, 64, s));
-  rf::unpack_latents_kernel<<<(H * W * 16 + 255) / 256, 256, 0, s>>>(
-      static_cast<const bf16*>(packed_latents), h->buf[x], H, W, scaling_factor, shift_factor);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYV(rf::unpack_latents_launch(static_cast<const bf16*>(packed_latents), h->buf[x], H, W, scaling_factor,
+                                    shift_factor, s));
   RF_TRYV(prep(h, y, H, W, 512, s));
   RF_TRYV(conv(h, h->conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
   std::swap(x, y);
@@ -952,13 +1028,7 @@ static int decode_body(rf_vae* h, const void* packed_latents, int height, int wi
     if (i < 3) {
       const int C = h->upconv[i].cin_pad;
       RF_TRYV(prep(h, y, 2 * H, 2 * W, C, s));
-      {
-        rf::ProfScope prof("vae_upsample", 0, 10.0 * H * W * C, s);
-        rf::upsample2x_kernel<<<grid_for(static_cast<long long>(4) * H * W * (C / 8)), 256, 0, s>>>(
-            h->buf[x], h->buf[y], H, W, C);
-      }
-      RF_CHECK_CUDA(cudaGetLastError());
-      rf::count_launch();
+      RF_TRYV(rf::upsample2x_launch(h->buf[x], h->buf[y], H, W, C, s));
       H *= 2;
       W *= 2;
       RF_TRYV(prep(h, x, H, W, C, s));
@@ -970,14 +1040,24 @@ static int decode_body(rf_vae* h, const void* packed_latents, int height, int wi
   RF_TRYV(group_norm(h, h->buf[x], h->buf[t1], H, W, h->norm_out, 1, 1, 1, s));
   RF_TRYV(prep(h, y, H, W, 128, s));
   RF_TRYV(conv(h, h->conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));
-  rf::postprocess_kernel<<<static_cast<int>((static_cast<long long>(H) * W + 255) / 256), 256, 0, s>>>(
-      h->buf[y], H, W, 128, out_u8_hwc, static_cast<bf16*>(out_bf16_chw));
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
-  return 0;
+  return rf::postprocess_launch(h->buf[y], H, W, 128, out_u8_hwc, static_cast<bf16*>(out_bf16_chw), s);
 }
 
 int rf_vae_missing_weights(rf_vae* h) { return vae_missing(h, ""); }
+
+}  // extern "C"
+
+int vae_mid_attention(rf_vae* h, int encoder, const bf16* x, bf16* out, int H, int W, cudaStream_t s) {
+  if (!h || !x || !out || H < 1 || W < 1 || H > 2048 || W > 2048) {
+    rf::set_error("vae_mid_attention: null argument or latent size outside [1, 2048]");
+    return -1;
+  }
+  if (vae_missing(h, encoder ? "encoder.mid_block.attentions." : "decoder.mid_block.attentions.") != 0) return -4;
+  RF_TRYV(ensure_workspace(h, 8 * H, 8 * W));
+  return mid_attention(h, encoder ? h->e_mid : h->mid, x, out, H, W, s);
+}
+
+extern "C" {
 
 /* image [H, W, 3] uint8 (or bf16 CHW in [-1, 1]) -> packed condition latents [(H/16)(W/16), 64]:
  * preprocess, encoder, posterior sample with caller-provided eps (NULL = mode), (z - shift) * scale,
@@ -1021,10 +1101,7 @@ static int encode_body(rf_vae* h, const uint8_t* image_u8_hwc, const void* image
   int x = 0, y = 1;
   const int t1 = 2, t2 = 3;
   RF_TRYV(prep(h, x, H, W, 64, s));
-  rf::image_to_nhwc_kernel<<<static_cast<int>((static_cast<long long>(H) * W + 255) / 256), 256, 0, s>>>(
-      image_u8_hwc, static_cast<const bf16*>(image_bf16_chw), h->buf[x], H, W);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYV(rf::image_to_nhwc_launch(image_u8_hwc, static_cast<const bf16*>(image_bf16_chw), h->buf[x], H, W, s));
   RF_TRYV(prep(h, y, H, W, 128, s));
   RF_TRYV(conv(h, h->e_conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
   std::swap(x, y);
@@ -1048,12 +1125,8 @@ static int encode_body(rf_vae* h, const uint8_t* image_u8_hwc, const void* image
   RF_TRYV(group_norm(h, h->buf[x], h->buf[t1], H, W, h->e_norm_out, 1, 1, 1, s));
   RF_TRYV(prep(h, y, H, W, 128, s));
   RF_TRYV(conv(h, h->e_conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));  // 32 moments (of 128)
-  rf::sample_pack_kernel<<<(H * W * 16 + 255) / 256, 256, 0, s>>>(
-      h->buf[y], 128, static_cast<const bf16*>(eps_bf16_chw), static_cast<bf16*>(packed_out), H, W,
-      scaling_factor, shift_factor);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
-  return 0;
+  return rf::sample_pack_launch(h->buf[y], 128, static_cast<const bf16*>(eps_bf16_chw),
+                                static_cast<bf16*>(packed_out), H, W, scaling_factor, shift_factor, s);
 }
 
 }  // extern "C"

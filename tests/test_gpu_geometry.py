@@ -53,6 +53,12 @@ def test_decode_ragged_matches_oracle(height, width):
     assert torch.isfinite(img_pt.float()).all()
     assert e_ours.mean() <= 1.5 * e_ref.mean() + 2e-3
     assert d.mean() <= 3.0 * e_ref.mean() + 2e-3
+    rim = torch.ones(height, width, dtype=torch.bool)
+    rim[1:-1, 1:-1] = False  # the image's one-pixel border on its own (a bad ring column hides in the whole mean)
+    print(f"  border: |ours-ref_bf16| mean {d[..., rim].mean():.4g} ; |ref-fp32| mean {e_ref[..., rim].mean():.4g} ; "
+          f"|ours-fp32| mean {e_ours[..., rim].mean():.4g}")
+    assert e_ours[..., rim].mean() <= 1.5 * e_ref[..., rim].mean() + 2e-3
+    assert d[..., rim].mean() <= 3.0 * e_ref[..., rim].mean() + 2e-3
     du = (img_u8.cpu().int() - vo.postprocess_uint8(want).int()).abs()
     print(f"  uint8: exact {float((du == 0).float().mean()):.3f}, max {int(du.max())}")
     assert (du <= 2).float().mean() > 0.99

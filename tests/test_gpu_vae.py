@@ -47,6 +47,12 @@ def test_decode_matches_oracle(height, width):
     assert torch.isfinite(img_pt.float()).all()
     assert e_ours.mean() <= 1.5 * e_ref.mean() + 2e-3
     assert d.mean() <= 3.0 * e_ref.mean() + 2e-3
+    rim = torch.ones(height, width, dtype=torch.bool)
+    rim[1:-1, 1:-1] = False  # the image's one-pixel border on its own (a bad ring column hides in the whole mean)
+    print(f"  border: |ours-ref_bf16| mean {d[..., rim].mean():.4g} ; |ref-fp32| mean {e_ref[..., rim].mean():.4g} ; "
+          f"|ours-fp32| mean {e_ours[..., rim].mean():.4g}")
+    assert e_ours[..., rim].mean() <= 1.5 * e_ref[..., rim].mean() + 2e-3
+    assert d[..., rim].mean() <= 3.0 * e_ref[..., rim].mean() + 2e-3
     u8_want = vo.postprocess_uint8(want)
     du = (img_u8.cpu().int() - u8_want.int()).abs()
     print(f"  uint8: exact {float((du == 0).float().mean()):.3f}, <=1 {float((du <= 1).float().mean()):.3f}, "
@@ -103,16 +109,6 @@ def test_captured_graphs_replay_the_eager_bits(monkeypatch):
     for i, (a, b) in enumerate(zip(graphed, eager)):
         assert torch.equal(a, b), f"call {i} differs between the graph replay and the eager launch sequence"
     assert torch.equal(graphed[0], graphed[5]) and not torch.equal(graphed[0], graphed[2])
-
-
-def test_postprocess_is_bit_exact_on_given_image():
-    """the uint8 conversion itself (x/2+0.5 in bf16, clamp, *255, round-half-even) is exact: feed the
-    oracle's own pre-quantisation image through the same formula"""
-    x = torch.linspace(-1.5, 1.5, 4096).to(torch.bfloat16).view(1, 1, 64, 64).expand(1, 3, 64, 64)
-    want = vo.postprocess_uint8(x)
-    t = (x / 2 + 0.5).clamp(0, 1).float()
-    got = torch.round(t * 255).to(torch.uint8).permute(0, 2, 3, 1)
-    assert torch.equal(want, got)
 
 
 @pytest.mark.parametrize("hw,out", [((1024, 1024), (512, 512)), ((256, 384), (128, 192)), ((100, 60), (37, 45))])
