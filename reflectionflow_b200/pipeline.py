@@ -153,6 +153,36 @@ class B200FluxPipeline:
         t.load_state_dict(state_dict)
         return cls(t)
 
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path, cache_dir=None, torch_dtype=torch.bfloat16,
+                        device="cuda:0", lora_rank: int = 0):
+        """DiffusionPipeline.from_pretrained(name, torch_dtype=.., cache_dir=..) (tts_reflectionflow.py:498-502)
+        for a FLUX.1-dev checkpoint in diffusers layout: a local directory, or a repo id already in the hub
+        cache (`cache_dir`, default $HF_HUB_CACHE / $HF_HOME).  Nothing is downloaded.  Transformer, VAE, T5 /
+        CLIP, their tokenizers and the scheduler all come from that directory; every config is checked before
+        any device memory is allocated.  `lora_rank` sizes the adapter slots (checkpoint.max_lora_rank reads it
+        from an adapter file); adapters load through load_lora_weights."""
+        from . import checkpoint as ck
+        from .text import B200TextEncoders
+        from .vae import B200AutoencoderKL
+        ck.check_dtype(torch_dtype)
+        root = ck.resolve(pretrained_model_name_or_path, cache_dir)
+        ck.check_model_index(root)
+        join = lambda comp, name="config.json": os.path.join(root, comp, name)  # noqa: E731
+        ck.dit_config(ck.read_json(join("transformer")))
+        ck.vae_config(ck.read_json(join("vae")))
+        ck.text_config(ck.read_json(join("text_encoder")), ck.read_json(join("text_encoder_2")))
+        sched = ck.scheduler_config(ck.read_json(join("scheduler", "scheduler_config.json")))
+        tokenizer, tokenizer_2 = ck.tokenizer_fns(root)
+        transformer = B200FluxTransformer2DModel.from_pretrained(join("transformer", ""), lora_rank=lora_rank,
+                                                                 device=device)
+        vae = B200AutoencoderKL.from_pretrained(join("vae", ""), device=device)
+        enc = B200TextEncoders.from_pretrained(join("text_encoder", ""), join("text_encoder_2", ""), device=device)
+        pipe = cls(transformer, text_encoder_hook=enc.as_hook(tokenizer, tokenizer_2), vae=vae)
+        pipe.scheduler = FlowMatchEulerDiscreteScheduler(**sched)
+        pipe.text_encoders = enc
+        return pipe
+
     def to(self, *a, **k):
         return self
 

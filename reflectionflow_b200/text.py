@@ -58,9 +58,26 @@ class B200TextEncoders:
         self._h = ctypes.c_void_p()
         self._bias: Dict[int, torch.Tensor] = {}
         self._rel_bias: Optional[torch.Tensor] = None
+        self.clip_eos_token_id = 2
         with torch.cuda.device(self.device):
             c = _TextCfg(**full)
             L.check(self._lib.rf_text_create(ctypes.byref(c), ctypes.byref(self._h)), "rf_text_create")
+
+    @classmethod
+    def from_pretrained(cls, text_encoder_dir: str, text_encoder_2_dir: str, device="cuda:0"):
+        """The diffusers `text_encoder/` (transformers CLIPTextModel) and `text_encoder_2/` (T5EncoderModel)
+        directories: shapes from their config.json (what the kernels do not implement is refused before the
+        handle is created), weights streamed from their safetensors.  `clip_eos_token_id` is CLIP's
+        eos_token_id, for the pooling rule of clip_encode."""
+        import os
+        from . import checkpoint as ck
+        fields, eos = ck.text_config(ck.read_json(os.path.join(text_encoder_dir, "config.json")),
+                                     ck.read_json(os.path.join(text_encoder_2_dir, "config.json")))
+        clip = ck.SafetensorsStream(text_encoder_dir, ck.clip_key)
+        t5 = ck.SafetensorsStream(text_encoder_2_dir, ck.t5_key)
+        enc = cls(device=device, **fields)
+        enc.clip_eos_token_id = eos
+        return enc.load_clip_state_dict(clip).load_t5_state_dict(t5)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -199,12 +216,12 @@ class B200TextEncoders:
         """text_encoder_hook for B200FluxPipeline: (prompt, prompt_2, max_len) -> (prompt_embeds,
         pooled).  tokenizer(prompts, max_len) -> LongTensor ids [B, 77] (CLIP BPE, padded);
         tokenizer_2(prompts, max_len) -> ids [B, max_len] (T5 sentencepiece, padded).  Mirrors
-        FluxPipeline._get_clip_prompt_embeds / _get_t5_prompt_embeds."""
+        FluxPipeline._get_clip_prompt_embeds / _get_t5_prompt_embeds; CLIP pools by clip_eos_token_id."""
 
         def hook(prompt, prompt_2, max_len):
             prompt = [prompt] if isinstance(prompt, str) else list(prompt)
             prompt_2 = prompt if prompt_2 is None else ([prompt_2] if isinstance(prompt_2, str) else list(prompt_2))
-            pooled, _ = self.clip_encode(tokenizer(prompt, 77))
+            pooled, _ = self.clip_encode(tokenizer(prompt, 77), self.clip_eos_token_id)
             embeds = self.t5_encode(tokenizer_2(prompt_2, max_len))
             return embeds, pooled
 

@@ -120,6 +120,16 @@ class B200FluxTransformer2DModel:
     def eval(self):
         return self
 
+    @classmethod
+    def from_pretrained(cls, transformer_dir: str, lora_rank: int = 0, device="cuda:0"):
+        """A diffusers `transformer/` directory: FluxDiTConfig from its config.json (values the kernels do not
+        implement are refused before the handle is created), weights streamed from its safetensors."""
+        import os
+        from . import checkpoint as ck
+        cfg = ck.dit_config(ck.read_json(os.path.join(transformer_dir, "config.json")))
+        stream = ck.SafetensorsStream(transformer_dir, ck.dit_key)
+        return cls(cfg, lora_rank=lora_rank, device=device).load_state_dict(stream)
+
     # ------------------------------------------------------------------ weights
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
         """`sd` uses diffusers' FluxTransformer2DModel keys.  Tensors may live anywhere; each is

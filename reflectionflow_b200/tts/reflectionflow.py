@@ -344,8 +344,11 @@ def _exchange_outputs(ctx: DistCtx, verifier_name: str, metric: str, cands: List
 
 def build_pipeline(config: dict, args, ctx: DistCtx):
     """DiffusionPipeline.from_pretrained(...).to("cuda") + load_lora_weights
-    (tts_reflectionflow.py:498-505).  Offline (--synthetic): random-init weights of the FLUX.1-dev
-    architecture, seeded identically on every rank, random LoRA, hash text embeddings."""
+    (tts_reflectionflow.py:498-505): the checkpoint `pretrained_model_name_or_path` names (a directory, or a
+    repo id in the hub cache under `cache_dir`), read from disk by every rank onto its own device, with the
+    adapter at `lora_path` (its rank sizes the transformer's LoRA slots).  Offline (--synthetic): random-init
+    weights of the FLUX.1-dev architecture, seeded identically on every rank, random LoRA, hash text
+    embeddings."""
     from ..config import FluxDiTConfig
     from ..pipeline import B200FluxPipeline
     pa = config["pipeline_args"]
@@ -355,8 +358,15 @@ def build_pipeline(config: dict, args, ctx: DistCtx):
         cfg = FluxDiTConfig(num_layers=nl, num_single_layers=ns)
     lora_path = pa.get("lora_path", None)
     if not getattr(args, "synthetic", False):
-        raise RuntimeError("no FLUX.1-dev checkpoint is reachable offline: run with --synthetic, or "
-                           "build B200FluxPipeline.from_state_dict(...) yourself and call sample()")
+        from ..checkpoint import max_lora_rank
+        pipe = B200FluxPipeline.from_pretrained(
+            pa["pretrained_model_name_or_path"], cache_dir=pa.get("cache_dir"), torch_dtype=pa.get("torch_dtype"),
+            device=ctx.device, lora_rank=max_lora_rank(lora_path) if lora_path is not None else 0)
+        if lora_path is not None:
+            pipe.transformer.lora_mode = getattr(args, "lora_mode", None) or "exact"
+            pipe.load_lora_weights(lora_path, adapter_name="reflection")
+        pipe.set_progress_bar_config(disable=True)
+        return pipe
     pipe = B200FluxPipeline.from_synthetic(cfg, seed=0, device=ctx.device,
                                            lora_rank=32 if lora_path is not None else 0, with_vae=True)
     if getattr(args, "text_encoders", "hash") == "native":

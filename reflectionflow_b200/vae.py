@@ -21,12 +21,12 @@ class _Cfg(dict):
 
 
 class B200AutoencoderKL:
-    def __init__(self, device="cuda:0"):
+    def __init__(self, device="cuda:0", scaling_factor: float = 0.3611, shift_factor: float = 0.1159):
         if not torch.cuda.is_available():
             raise L.RFError("B200AutoencoderKL needs a CUDA device; there is no CPU fallback")
         self.device = torch.device(device)
         self.dtype = torch.bfloat16
-        self.config = _Cfg(scaling_factor=0.3611, shift_factor=0.1159, latent_channels=16,
+        self.config = _Cfg(scaling_factor=scaling_factor, shift_factor=shift_factor, latent_channels=16,
                            block_out_channels=(128, 256, 512, 512))
         self._lib = L.load()
         self._h = ctypes.c_void_p()
@@ -43,6 +43,17 @@ class B200AutoencoderKL:
             self.close()
         except Exception:
             pass
+
+    @classmethod
+    def from_pretrained(cls, vae_dir: str, device="cuda:0"):
+        """A diffusers `vae/` directory: scaling / shift factors from its config.json (any other shape than the
+        FLUX VAE's is refused before the handle is created), weights streamed from its safetensors (the FLUX
+        VAE ships in fp32; they are cast to bf16 on the host)."""
+        import os
+        from . import checkpoint as ck
+        factors = ck.vae_config(ck.read_json(os.path.join(vae_dir, "config.json")))
+        stream = ck.SafetensorsStream(vae_dir, ck.vae_key)
+        return cls(device, **factors).load_state_dict(stream)
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True):
         """diffusers AutoencoderKL keys (`decoder.*` and `encoder.*`)."""
