@@ -103,6 +103,15 @@ int rf_op_timestep_embed(const void* t, float pre_scale, void* out, int batch, v
 int rf_op_euler_step(void* x, const void* v, const float* sigmas, const int* step, int n,
                      void* stream);
 
+/* Image classifier-free guidance followed by the Euler step (generate.py:250-276):
+ *   v = unc_pred + s * (noise_pred - unc_pred)  as torch evaluates it on bf16 tensors with a Python scalar,
+ *       i.e. v = bf16(u + bf16(float(s) * bf16(c - u)))  (s rounded to fp32, not bf16 or double);
+ *   x = bf16(float(x) + (sigmas[i+1]-sigmas[i]) * float(v)).
+ * v_cond (c) / v_uncond (u): bf16 [n]; scale: DEVICE fp32 s; sigmas: device fp32; step: device int32 i;
+ * n a multiple of 8. */
+int rf_op_image_guidance_step(void* x, const void* v_cond, const void* v_uncond, const float* scale,
+                              const float* sigmas, const int* step, int n, void* stream);
+
 /* Pillow-compatible BICUBIC resize of a uint8 HWC image (Image.resize default filter): the
  * parent -> condition resize of tts/tts_reflectionflow.py:276-277.  Integer resampling tables
  * (bounds [out,2] = (first, count), coef [out, ksize], 22 fractional bits) come from the host
@@ -209,6 +218,22 @@ int rf_dit_forward(rf_dit* h, const void* latents, const void* txt, const void* 
 int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
                    const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
                    float guidance_scale, const void* cond_latents, void* stream);
+
+/* rf_dit_denoise with image classifier-free guidance over the condition stream (generate.py:250-272,
+ * `image_guidance_scale` s != 1).  Each step i runs two forwards on the same latents, prompt, pooled and timestep:
+ *   c = forward(cond_latents,        guidance = guidance_scale)
+ *   u = forward(uncond_latents[:, i], guidance = 1.0 (bf16(1) * 1000 in the model))
+ * then v = u + s * (c - u) and the Euler step, as rf_op_image_guidance_step.  The reference's uncond input is
+ * `condition.encode(self, empty=True)[0]`, which re-encodes the REAL condition image (condition.py:121 overwrites
+ * the black-image encode of :118): a fresh VAE posterior sample of the same parent per step, supplied here as
+ * uncond_latents [B, n_steps, n_cond, 64] (device bf16).  The condition modulation (cond_temb) does not depend
+ * on guidance and is shared by both branches.  Needs a geometry with n_cond > 0 and a model with
+ * guidance_embeds.  The guided step is captured into a CUDA graph of its own; s lives in device memory, so
+ * calls with another s, and calls alternating with rf_dit_denoise, replay no stale graph. */
+int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
+                                  const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                                  float guidance_scale, const void* cond_latents, const void* uncond_latents,
+                                  float image_guidance_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * FLUX VAE decoder (next-tier row: `vae.decode` + `image_processor.postprocess`,

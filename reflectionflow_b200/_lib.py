@@ -48,6 +48,8 @@ def _declare(lib):
     lib.rf_op_timestep_embed.argtypes = [vp, cf, vp, ci, vp]
     lib.rf_op_euler_step.restype = ci
     lib.rf_op_euler_step.argtypes = [vp, vp, vp, vp, ci, vp]
+    lib.rf_op_image_guidance_step.restype = ci
+    lib.rf_op_image_guidance_step.argtypes = [vp, vp, vp, vp, vp, vp, ci, vp]
     lib.rf_op_resize_u8.restype = ci
     lib.rf_op_resize_u8.argtypes = [vp, ci, ci, vp, vp, ci, ci, vp, vp, ci, vp, vp, ci, vp]
     lib.rf_dbg_force_gemm_v1.restype = None
@@ -98,6 +100,8 @@ def _declare(lib):
         lib.rf_dit_forward.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.rf_dit_denoise.restype = ci
         lib.rf_dit_denoise.argtypes = [vp, vp, vp, vp, vp, vp, ci, cf, vp, vp]
+        lib.rf_dit_denoise_image_guidance.restype = ci
+        lib.rf_dit_denoise_image_guidance.argtypes = [vp, vp, vp, vp, vp, vp, ci, cf, vp, vp, cf, vp]
 
 
 def load():

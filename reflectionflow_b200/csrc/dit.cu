@@ -99,6 +99,13 @@ struct SingleBlk {
 
 }  // namespace
 
+// one denoise step captured into a CUDA graph
+struct StepGraph {
+  cudaGraphExec_t exec = nullptr;
+  int64_t kernels = 0;      // kernel launches inside the step
+  double call_scale = 1.0;  // call_scale the step was built with (kernel parameters, launch list)
+};
+
 struct rf_dit {
   rf_dit_config cfg;
   int D = 0;
@@ -149,11 +156,14 @@ struct rf_dit {
   // front): MOD_ALL [n_steps, n_mod]; the captured step only selects its row
   bf16 *s_mod_all = nullptr, *s_temb_ws = nullptr;
   int s_cap_steps = 0;
-  cudaGraphExec_t graph_exec = nullptr;
+  // image guidance (rf_dit_denoise_image_guidance): the uncond branch's table MOD_ALL at guidance bf16(1) (same
+  // layout, s_cap_steps_u rows), its condition input U_i and noise prediction, and the scale s (device fp32)
+  bf16 *s_mod_all_u = nullptr, *s_ucond = nullptr, *s_vu = nullptr;
+  float* s_igs = nullptr;
+  int s_cap_steps_u = 0;
+  StepGraph graph, graph_ig;  // the captured step of rf_dit_denoise / of the guided loop
   cudaStream_t own_stream = nullptr;  // capture is illegal on the legacy default stream
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-  int64_t graph_kernels = 0;  // kernel launches inside one captured step
-  double graph_call_scale = 1.0;  // call_scale the captured step was built with (kernel parameters, launch list)
 };
 
 namespace {
@@ -768,9 +778,11 @@ int alloc_lora_ws(rf_dit* h, int rows) {
 bool merged_current(const rf_dit* h) { return h->lora_merged && h->merged_call_scale == h->call_scale; }
 
 void drop_graph(rf_dit* h) {
-  if (h->graph_exec) {
-    cudaGraphExecDestroy(h->graph_exec);
-    h->graph_exec = nullptr;
+  for (StepGraph* g : {&h->graph, &h->graph_ig}) {
+    if (g->exec) {
+      cudaGraphExecDestroy(g->exec);
+      g->exec = nullptr;
+    }
   }
 }
 void free_geometry(rf_dit* h) {
@@ -782,6 +794,8 @@ void free_geometry(rf_dit* h) {
   h->s_cap_steps = 0;
   h->s_tsteps = nullptr;
   h->s_sigmas = nullptr;
+  h->s_cap_steps_u = 0;
+  h->s_mod_all_u = nullptr;
 }
 
 }  // namespace
@@ -1130,9 +1144,16 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     if (!(p = A(static_cast<size_t>(batch) * 2 + 16))) return -2; h->s_guid = static_cast<bf16*>(p);
     if (!(p = A(16))) return -2; h->s_zero_one = static_cast<bf16*>(p);
     if (!(p = A(16))) return -2; h->s_step = static_cast<int*>(p);
+    if (n_cond > 0) {  // image guidance needs a condition stream
+      if (!(p = A(static_cast<size_t>(n_cond) * C * 2))) return -2; h->s_ucond = static_cast<bf16*>(p);
+      if (!(p = A(static_cast<size_t>(n_img) * C * 2))) return -2; h->s_vu = static_cast<bf16*>(p);
+      if (!(p = A(16))) return -2; h->s_igs = static_cast<float*>(p);
+    }
     h->s_cap_steps = 0;
     h->s_tsteps = nullptr;
     h->s_sigmas = nullptr;
+    h->s_cap_steps_u = 0;
+    h->s_mod_all_u = nullptr;
     const uint16_t zo[2] = {0x0000, 0x3F80};  // bf16 0.0, 1.0
     RF_CHECK_CUDA(cudaMemcpy(h->s_zero_one, zo, sizeof(zo), cudaMemcpyHostToDevice));
   }
@@ -1222,16 +1243,53 @@ int rf_dit_forward(rf_dit* h, const void* latents, const void* txt, const void* 
   return 0;
 }
 
-int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
-                   const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
-                   float guidance_scale, const void* cond_latents, void* stream) {
-  int rc = check_ready(h, "rf_dit_denoise", static_cast<cudaStream_t>(stream));
-  if (rc) return rc;
-  if (!latents_inout || !txt || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 ||
-      (h->n_cond > 0 && !cond_latents)) {
-    rf::set_error("rf_dit_denoise: bad argument");
-    return -1;
+// Capture one step of the denoise loop into g: forward -> Euler update -> step counter, or with image guidance
+// forward (cond) -> forward (uncond: its own modulation table, condition input U_i) -> guidance + Euler -> counter.
+static int capture_step(rf_dit* h, bool guided, StepGraph* g, cudaStream_t s) {
+  const int C = h->cfg.in_channels;
+  g->call_scale = h->call_scale;
+  cudaGraph_t graph = nullptr;
+  const int64_t launches_before = rf::launch_count();
+  RF_CHECK_CUDA(cudaStreamSynchronize(s));
+  RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  int erc = enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_guid,
+                            h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s, h->s_mod_all);
+  if (guided) {
+    if (!erc) erc = enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_zero_one + 1,
+                                    h->s_ucond, h->s_vu, s, h->s_mod_all_u);
+    if (!erc) erc = rf::image_guidance_step_launch(h->s_lat, h->s_v, h->s_vu, h->s_igs, h->s_sigmas, h->s_step,
+                                                   h->n_img * C, s);
+  } else if (!erc) {
+    erc = rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s);
   }
+  if (!erc) erc = rf::advance_step_launch(h->s_step, s);
+  cudaError_t ce = cudaStreamEndCapture(s, &graph);
+  if (erc || ce != cudaSuccess) {
+    if (graph) cudaGraphDestroy(graph);
+    if (!erc) {
+      rf::set_error(std::string("graph capture failed: ") + cudaGetErrorString(ce));
+      erc = -2;
+    }
+    return erc;
+  }
+  g->kernels = rf::launch_count() - launches_before;
+  rf::count_launch(static_cast<int>(-g->kernels));  // captured, not executed
+  ce = cudaGraphInstantiate(&g->exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ce != cudaSuccess) {
+    g->exec = nullptr;
+    rf::set_error(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
+    return -2;
+  }
+  return 0;
+}
+
+// rf_dit_denoise, and with uncond_latents != nullptr rf_dit_denoise_image_guidance (arguments checked by the caller)
+static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
+                        const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                        float guidance_scale, const void* cond_latents, const bf16* uncond_latents,
+                        float image_guidance_scale, void* stream) {
+  const bool guided = uncond_latents != nullptr;
   // The loop runs on a handle-owned stream (graph capture is not permitted on the legacy default
   // stream callers often pass); it is ordered after / before the caller's stream with events, so
   // the call still only enqueues work.
@@ -1258,12 +1316,23 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     h->s_cap_steps = n_steps;
     drop_graph(h);  // graph referenced the old arrays
   }
+  if (guided && n_steps > h->s_cap_steps_u) {
+    void* p = nullptr;
+    if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
+    h->s_mod_all_u = static_cast<bf16*>(p);
+    h->s_cap_steps_u = n_steps;
+    drop_graph(h);
+  }
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_tsteps, timesteps_bf16_host, static_cast<size_t>(n_steps) * 2,
                                 cudaMemcpyHostToDevice, s));
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_sigmas, sigmas_host, static_cast<size_t>(n_steps + 1) * 4,
                                 cudaMemcpyHostToDevice, s));
   const bf16 gb = __float2bfloat16_rn(guidance_scale);
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_guid, &gb, 2, cudaMemcpyHostToDevice, s));
+  if (guided)
+    RF_CHECK_CUDA(cudaMemcpyAsync(h->s_igs, &image_guidance_scale, 4, cudaMemcpyHostToDevice, s));
+  StepGraph* g = guided ? &h->graph_ig : &h->graph;
+  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
 
   for (int b = 0; b < h->batch; ++b) {
     bf16* lat_b = static_cast<bf16*>(latents_inout) + static_cast<int64_t>(b) * h->n_img * C;
@@ -1286,44 +1355,21 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
     }
     RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, h->s_pooled, (h->flags & 1) != 0, true, h->s_mod_all,
                     h->s_temb_ws, s));
+    // the uncond branch: guidance = torch.ones_like(guidance) -> bf16(1) * 1000 in the model (generate.py:262)
+    if (guided)
+      RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_zero_one + 1, h->s_pooled, (h->flags & 1) != 0, true,
+                      h->s_mod_all_u, h->s_temb_ws, s));
     RF_CHECK_CUDA(cudaMemsetAsync(h->s_step, 0, sizeof(int), s));
     // the captured step holds the LoRA scalings as kernel parameters (and skips the terms a zero scaling
     // removes): a changed call scale is re-captured
-    if (h->graph_exec && h->graph_call_scale != h->call_scale) drop_graph(h);
-    if (!h->graph_exec) {
-      h->graph_call_scale = h->call_scale;
-      // capture one step: forward -> Euler update -> step counter
-      cudaGraph_t graph = nullptr;
-      const int64_t launches_before = rf::launch_count();
-      RF_CHECK_CUDA(cudaStreamSynchronize(s));
-      RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-      int erc = enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step,
-                                h->s_guid, h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s,
-                                h->s_mod_all);
-      if (!erc) erc = rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s);
-      if (!erc) erc = rf::advance_step_launch(h->s_step, s);
-      cudaError_t ce = cudaStreamEndCapture(s, &graph);
-      if (erc || ce != cudaSuccess) {
-        if (graph) cudaGraphDestroy(graph);
-        if (!erc) {
-          rf::set_error(std::string("graph capture failed: ") + cudaGetErrorString(ce));
-          erc = -2;
-        }
-        return erc;
-      }
-      h->graph_kernels = rf::launch_count() - launches_before;
-      rf::count_launch(static_cast<int>(-h->graph_kernels));  // captured, not executed
-      ce = cudaGraphInstantiate(&h->graph_exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        h->graph_exec = nullptr;
-        rf::set_error(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
-        return -2;
-      }
-    }
+    if (g->exec && g->call_scale != h->call_scale) drop_graph(h);
+    if (!g->exec) RF_TRY(capture_step(h, guided, g, s));
     for (int i = 0; i < n_steps; ++i) {
-      RF_CHECK_CUDA(cudaGraphLaunch(h->graph_exec, s));
-      rf::count_launch(static_cast<int>(h->graph_kernels));
+      if (guided)  // U_i of this sample: [B, n_steps, n_cond, 64]
+        RF_CHECK_CUDA(cudaMemcpyAsync(h->s_ucond, uncond_latents + (static_cast<size_t>(b) * n_steps + i) * cond_elems,
+                                      cond_elems * 2, cudaMemcpyDeviceToDevice, s));
+      RF_CHECK_CUDA(cudaGraphLaunch(g->exec, s));
+      rf::count_launch(static_cast<int>(g->kernels));
     }
     RF_CHECK_CUDA(cudaMemcpyAsync(lat_b, h->s_lat, static_cast<size_t>(h->n_img) * C * 2,
                                   cudaMemcpyDeviceToDevice, s));
@@ -1331,6 +1377,43 @@ int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* 
   RF_CHECK_CUDA(cudaEventRecord(h->ev_out, s));
   RF_CHECK_CUDA(cudaStreamWaitEvent(caller, h->ev_out, 0));
   return 0;
+}
+
+int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
+                   const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                   float guidance_scale, const void* cond_latents, void* stream) {
+  int rc = check_ready(h, "rf_dit_denoise", static_cast<cudaStream_t>(stream));
+  if (rc) return rc;
+  if (!latents_inout || !txt || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 ||
+      (h->n_cond > 0 && !cond_latents)) {
+    rf::set_error("rf_dit_denoise: bad argument");
+    return -1;
+  }
+  return denoise_loop(h, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale,
+                      cond_latents, nullptr, 1.0f, stream);
+}
+
+int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
+                                  const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                                  float guidance_scale, const void* cond_latents, const void* uncond_latents,
+                                  float image_guidance_scale, void* stream) {
+  int rc = check_ready(h, "rf_dit_denoise_image_guidance", static_cast<cudaStream_t>(stream));
+  if (rc) return rc;
+  if (!latents_inout || !txt || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 || !cond_latents ||
+      !uncond_latents) {
+    rf::set_error("rf_dit_denoise_image_guidance: bad argument");
+    return -1;
+  }
+  if (h->n_cond <= 0 || !h->cfg.guidance_embeds) {
+    rf::set_error("rf_dit_denoise_image_guidance: needs a condition stream (n_cond > 0) and guidance_embeds");
+    return -1;
+  }
+  if (!std::isfinite(image_guidance_scale)) {
+    rf::set_error("rf_dit_denoise_image_guidance: image_guidance_scale must be finite");
+    return -1;
+  }
+  return denoise_loop(h, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale,
+                      cond_latents, static_cast<const bf16*>(uncond_latents), image_guidance_scale, stream);
 }
 
 }  // extern "C"

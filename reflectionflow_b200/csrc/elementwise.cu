@@ -347,6 +347,52 @@ int euler_step_launch(bf16* x, const bf16* v, const float* sigmas, const int* st
   return 0;
 }
 
+// image classifier-free guidance (generate.py:270) then the Euler step above:
+//   v = bf16( u + bf16( s * bf16(c - u) ) )   — torch's bf16 ops with the Python scalar s taken as fp32
+//   x = bf16( float(x) + (sigma_{i+1} - sigma_i) * float(v) )
+__global__ void image_guidance_step_kernel(bf16* __restrict__ x, const bf16* __restrict__ vc,
+                                           const bf16* __restrict__ vu, const float* __restrict__ scale,
+                                           const float* __restrict__ sigmas, const int* __restrict__ step, int n) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int i = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if (i >= n) return;
+  const int s = *step;
+  const float dt = __fsub_rn(sigmas[s + 1], sigmas[s]);
+  const float g = *scale;
+  uint4 ux = *reinterpret_cast<const uint4*>(x + i);
+  uint4 uc = __ldg(reinterpret_cast<const uint4*>(vc + i));
+  uint4 uu = __ldg(reinterpret_cast<const uint4*>(vu + i));
+  uint32_t xs[4] = {ux.x, ux.y, ux.z, ux.w}, cs[4] = {uc.x, uc.y, uc.z, uc.w}, us[4] = {uu.x, uu.y, uu.z, uu.w};
+  uint32_t os[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float2 xf = unpack_bf16x2(xs[q]), cf = unpack_bf16x2(cs[q]), uf = unpack_bf16x2(us[q]);
+    float v[2], xo[2];
+    const float c2[2] = {cf.x, cf.y}, u2[2] = {uf.x, uf.y}, x2[2] = {xf.x, xf.y};
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float d = bf16_round(__fsub_rn(c2[e], u2[e]));
+      v[e] = bf16_round(__fadd_rn(u2[e], bf16_round(__fmul_rn(g, d))));
+      xo[e] = __fadd_rn(x2[e], __fmul_rn(dt, v[e]));
+    }
+    os[q] = pack_bf16x2(xo[0], xo[1]);
+  }
+  *reinterpret_cast<uint4*>(x + i) = make_uint4(os[0], os[1], os[2], os[3]);
+}
+int image_guidance_step_launch(bf16* x, const bf16* v_cond, const bf16* v_uncond, const float* scale,
+                               const float* sigmas, const int* step, int n, cudaStream_t stream) {
+  if (n % 8 != 0) {
+    set_error("image_guidance_step: n must be a multiple of 8");
+    return -1;
+  }
+  const int threads = n / 8;
+  RF_CHECK_CUDA(launch_pdl(image_guidance_step_kernel, dim3((threads + 255) / 256), dim3(256), 0, stream, x, v_cond,
+                           v_uncond, scale, sigmas, step, n));
+  count_launch();
+  return 0;
+}
+
 __global__ void advance_step_kernel(int* step) {
   pdl_launch_dependents();
   pdl_wait();

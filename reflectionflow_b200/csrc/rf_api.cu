@@ -430,4 +430,15 @@ int rf_op_euler_step(void* x, const void* v, const float* sigmas, const int* ste
                                static_cast<cudaStream_t>(stream));
 }
 
+int rf_op_image_guidance_step(void* x, const void* v_cond, const void* v_uncond, const float* scale,
+                              const float* sigmas, const int* step, int n, void* stream) {
+  if (!x || !v_cond || !v_uncond || !scale || !sigmas || !step) {
+    rf::set_error("rf_op_image_guidance_step: null operand");
+    return -1;
+  }
+  return rf::image_guidance_step_launch(static_cast<bf16*>(x), static_cast<const bf16*>(v_cond),
+                                        static_cast<const bf16*>(v_uncond), scale, sigmas, step, n,
+                                        static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -166,6 +166,9 @@ int add3_launch(const bf16* a, const bf16* b, const bf16* c, bf16* out, int n,
 // x = bf16(float(x) + dt * float(v))
 int euler_step_launch(bf16* x, const bf16* v, const float* sigmas, const int* step, int n,
                       cudaStream_t stream);
+// x = bf16(float(x) + dt * float(v)), v = bf16(u + bf16(scale * bf16(c - u))); scale: device fp32
+int image_guidance_step_launch(bf16* x, const bf16* v_cond, const bf16* v_uncond, const float* scale,
+                               const float* sigmas, const int* step, int n, cudaStream_t stream);
 int copy_rows_launch(const bf16* src, int lds, bf16* dst, int ldd, int rows, int cols,
                      cudaStream_t stream);
 // dst[r * ldd + c] = bf16(dst[r * ldd + c] + bf16(src[r * lds + c] * scale)) for r < rows, c < cols

@@ -52,11 +52,18 @@ class Condition:
     """train_flux/flux/condition.py:24-132 for the `cot` type: a parent image whose VAE latents
     join the sequence as condition tokens.  `latents` ([1, n, 64] packed, already shifted/scaled)
     may be given explicitly — the reference samples them from the VAE posterior with no
-    generator (pipeline_tools.py:10), which is not reproducible."""
+    generator (pipeline_tools.py:10), which is not reproducible.
+
+    Image guidance (generate(..., image_guidance_scale != 1)) re-encodes the condition every step: the reference's
+    `condition.encode(self, empty=True)` encodes the real image again (condition.py:121), a fresh posterior sample.
+    With explicit `latents`, `uncond_latents` ([n_steps, *latents.shape]) gives those samples U_i; without it U_i =
+    `latents`.  From an image, each U_i draws its posterior noise after the one of `latents`, from `generator` (else
+    the global CPU RNG)."""
 
     def __init__(self, condition_type: str = "cot", raw_img=None, condition=None, mask=None,
                  position_delta=None, latents: Optional[torch.Tensor] = None,
-                 eps: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None):
+                 eps: Optional[torch.Tensor] = None, generator: Optional[torch.Generator] = None,
+                 uncond_latents: Optional[torch.Tensor] = None):
         if condition_type not in condition_dict:
             raise NotImplementedError(f"Condition type {condition_type} not implemented")
         assert mask is None, "Mask not supported yet"
@@ -68,6 +75,9 @@ class Condition:
         self.position_delta = position_delta
         self.latents = latents
         self.eps, self.generator = eps, generator  # posterior noise of the VAE encode (explicit)
+        if uncond_latents is not None and latents is None:
+            raise ValueError("uncond_latents go with explicit latents; a Condition from an image samples them")
+        self.uncond_latents = uncond_latents
 
     def get_condition(self, condition_type: str, raw_img):
         """condition.py:43-80: raw image -> condition image.  "depth" needs the depth-anything network (not reachable
@@ -111,6 +121,20 @@ class Condition:
             ids[:, 2] += self.position_delta[1]
         type_id = torch.ones_like(ids[:, :1]) * self.type_id
         return tokens, ids, type_id
+
+    def encode_uncond(self, pipe: "B200FluxPipeline", n_steps: int) -> torch.Tensor:
+        """The uncond condition tokens of an image-guided loop, [B, n_steps, n, 64]: row i is step i's
+        `condition.encode(self, empty=True)[0]` (generate.py:251).  Call after `encode`."""
+        if self.latents is not None:
+            c0 = self.latents
+            if self.uncond_latents is None:
+                return c0[:, None].expand(c0.shape[0], n_steps, *c0.shape[1:])
+            if tuple(self.uncond_latents.shape) != (n_steps,) + tuple(c0.shape):
+                raise ValueError(f"uncond_latents has shape {tuple(self.uncond_latents.shape)}, expected "
+                                 f"{(n_steps,) + tuple(c0.shape)} (steps, *latents.shape)")
+            return self.uncond_latents.transpose(0, 1)
+        return torch.stack([pipe.encode_images(self.condition, generator=self.generator)[0]
+                            for _ in range(n_steps)], dim=1)
 
 
 class B200FluxPipeline:
@@ -341,7 +365,8 @@ class B200FluxPipeline:
     # ------------------------------------------------------------------ the denoise call
     def _denoise(self, latents, prompt_embeds, pooled, text_ids, image_ids, num_inference_steps,
                  guidance_scale, timesteps=None, condition_latents=None, condition_ids=None,
-                 model_config=None, condition_scale: float = 1.0):
+                 model_config=None, condition_scale: float = 1.0, image_guidance_scale: float = 1.0,
+                 uncond_latents=None):
         if timesteps is not None:
             raise NotImplementedError("custom `timesteps` are not supported (the reference passes sigmas)")
         sigmas = np.linspace(1.0, 1 / num_inference_steps, num_inference_steps)
@@ -355,7 +380,10 @@ class B200FluxPipeline:
         t_in = ts.to(self.dtype) / 1000
         return self.transformer.denoise(latents, prompt_embeds, pooled, t_in, self.scheduler.sigmas,
                                         guidance_scale, image_ids, text_ids, condition_latents,
-                                        condition_ids, model_config, condition_scale)
+                                        condition_ids, model_config, condition_scale,
+                                        **({} if image_guidance_scale == 1.0 else dict(
+                                            image_guidance_scale=image_guidance_scale,
+                                            uncond_condition_latents=uncond_latents)))
 
     def _finish(self, latents, height, width, output_type, return_dict):
         if output_type == "latent":
@@ -462,10 +490,13 @@ def generate(pipeline: B200FluxPipeline, conditions: List[Condition] = None, con
     """train_flux/flux/generate.py:75-321 (entry B): FluxPipeline.__call__ + one condition stream.
     Same keyword surface (prepare_params, generate.py:25-65); defaults 512x512 / 28 steps / 3.5."""
     model_config = model_config or get_config(config_path).get("model", {}) or {}
-    if image_guidance_scale != 1.0:
-        raise NotImplementedError("image_guidance_scale != 1 is broken upstream (SURVEY App. B.3) "
-                                  "and unused by the tts path")
     self = pipeline
+    guided = image_guidance_scale != 1.0  # generate.py:250-272
+    if guided and conditions is None:  # a NameError upstream (`condition` is unbound)
+        raise ValueError("image_guidance_scale != 1 guides over the condition stream: pass a condition")
+    if guided and not self.transformer.config.guidance_embeds:  # a TypeError upstream (ones_like(None))
+        raise ValueError("image_guidance_scale != 1 runs its uncond branch at guidance 1: it needs a model with "
+                         "guidance_embeds=True")
     prompt = params.get("prompt")
     prompt_2 = params.get("prompt_2")
     height = params.get("height", 512) or self.default_sample_size * self.vae_scale_factor
@@ -515,10 +546,11 @@ def generate(pipeline: B200FluxPipeline, conditions: List[Condition] = None, con
             ids.append(i)
         cond_lat = torch.cat(toks, dim=1)
         cond_ids = torch.cat(ids, dim=0)
+    unc_lat = conditions[-1].encode_uncond(self, num_inference_steps) if guided else None
     # joint_attention_kwargs["scale"] reaches every step of the loop (generate.py:246 -> transformer.py:73-81)
     with lora_scale(self.transformer, self._joint_attention_kwargs):
         latents = self._denoise(latents, prompt_embeds, pooled_prompt_embeds, text_ids, latent_image_ids,
                                 num_inference_steps, guidance_scale, params.get("timesteps"), cond_lat,
-                                cond_ids, model_config, condition_scale)
+                                cond_ids, model_config, condition_scale, image_guidance_scale, unc_lat)
     return self._finish(latents, height, width, params.get("output_type", "pil"),
                         params.get("return_dict", True))

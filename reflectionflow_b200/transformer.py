@@ -13,6 +13,7 @@ kernels.  There is no PyTorch fallback: without librf_b200.so or without a GPU t
 from __future__ import annotations
 
 import ctypes
+import math
 from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Any, Dict, Optional
@@ -323,25 +324,56 @@ class B200FluxTransformer2DModel:
     def denoise(self, latents, prompt_embeds, pooled, timesteps_bf16: torch.Tensor,
                 sigmas_f32: torch.Tensor, guidance_scale: float, img_ids, txt_ids,
                 condition_latents=None, condition_ids=None, model_config=None,
-                condition_scale: float = 1.0) -> torch.Tensor:
-        """Whole denoise loop on the device (rf_dit_denoise): one CUDA graph per step, replayed."""
+                condition_scale: float = 1.0, image_guidance_scale: float = 1.0,
+                uncond_condition_latents=None) -> torch.Tensor:
+        """Whole denoise loop on the device (rf_dit_denoise): one CUDA graph per step, replayed.
+
+        `image_guidance_scale` s != 1: image classifier-free guidance over the condition stream (generate.py:250-272,
+        rf_dit_denoise_image_guidance).  Every step adds a forward with the condition latents U_i of
+        `uncond_condition_latents` [B, n_steps, n_cond, 64] and guidance 1, and steps on u + s * (c - u).  Without
+        them U_i = condition_latents for every step.  s == 1 is the plain loop and ignores them."""
         B = latents.shape[0]
+        ts = timesteps_bf16.detach().to("cpu", torch.bfloat16).contiguous().view(torch.int16)
+        sg = sigmas_f32.detach().to("cpu", torch.float32).contiguous()
+        n = ts.numel()
+        assert sg.numel() == n + 1
+        guided = image_guidance_scale != 1.0
+        if guided:
+            if not math.isfinite(image_guidance_scale):
+                raise ValueError(f"image_guidance_scale must be finite, got {image_guidance_scale}")
+            if condition_latents is None or condition_ids is None:
+                raise ValueError("image_guidance_scale != 1 guides over the condition stream: it needs a condition")
+            if not self.cfg.guidance_embeds:
+                raise ValueError("image_guidance_scale != 1 runs its uncond branch at guidance 1, which needs a model "
+                                 "with guidance_embeds=True")
+            shape = (B, condition_ids.shape[-2], self.cfg.in_channels)
+            if tuple(condition_latents.shape) != shape:
+                raise ValueError(f"condition_latents has shape {tuple(condition_latents.shape)}, image guidance "
+                                 f"needs {shape} (batch, condition tokens, channels)")
+            if uncond_condition_latents is None:
+                uncond_condition_latents = condition_latents[:, None].expand(B, n, *shape[1:])
+            if tuple(uncond_condition_latents.shape) != (B, n) + shape[1:]:
+                raise ValueError(f"uncond_condition_latents has shape {tuple(uncond_condition_latents.shape)}, "
+                                 f"expected {(B, n) + shape[1:]} (batch, steps, condition tokens, channels)")
         self.prepare(B, txt_ids, img_ids, condition_ids, model_config, condition_scale)
         dev = self.device
         lat = _bf16c(latents, dev).clone()
         txt = _bf16c(prompt_embeds, dev)
         pool = _bf16c(pooled, dev)
         cond = _bf16c(condition_latents, dev) if condition_latents is not None else None
-        ts = timesteps_bf16.detach().to("cpu", torch.bfloat16).contiguous().view(torch.int16)
-        sg = sigmas_f32.detach().to("cpu", torch.float32).contiguous()
-        n = ts.numel()
-        assert sg.numel() == n + 1
         with torch.cuda.device(dev):
-            L.check(self._lib.rf_dit_denoise(self._h, L.ptr(lat), L.ptr(txt), L.ptr(pool),
-                                             ctypes.c_void_p(ts.data_ptr()),
-                                             ctypes.c_void_p(sg.data_ptr()), n,
-                                             ctypes.c_float(guidance_scale), L.ptr(cond),
-                                             L.cur_stream()), "rf_dit_denoise")
+            if guided:
+                unc = _bf16c(uncond_condition_latents, dev)
+                L.check(self._lib.rf_dit_denoise_image_guidance(
+                    self._h, L.ptr(lat), L.ptr(txt), L.ptr(pool), ctypes.c_void_p(ts.data_ptr()),
+                    ctypes.c_void_p(sg.data_ptr()), n, ctypes.c_float(guidance_scale), L.ptr(cond), L.ptr(unc),
+                    ctypes.c_float(image_guidance_scale), L.cur_stream()), "rf_dit_denoise_image_guidance")
+            else:
+                L.check(self._lib.rf_dit_denoise(self._h, L.ptr(lat), L.ptr(txt), L.ptr(pool),
+                                                 ctypes.c_void_p(ts.data_ptr()),
+                                                 ctypes.c_void_p(sg.data_ptr()), n,
+                                                 ctypes.c_float(guidance_scale), L.ptr(cond),
+                                                 L.cur_stream()), "rf_dit_denoise")
             torch.cuda.current_stream().synchronize()  # ts/sg host buffers must outlive the copies
         return lat
 

@@ -4,8 +4,9 @@
 Env: LAYERS=double,single (default 19,38), LORA=0|1, LORA_MODE=exact|merged, LATENT_LORA=1 (the LoRA also acts on the
 image and text tokens, model_config["latent_lora"]), LORA_RANK (default 32, up to 128), LORA_SCALE (default 1: the
 call's joint_attention_kwargs["scale"]), LORA_TARGETS=config|all-linear (default config: the adapter covers the
-Linears of train_flux/config.yaml:53; all-linear: every Linear of the transformer), STEPS.  Prints the card name and
-power limit with the timing."""
+Linears of train_flux/config.yaml:53; all-linear: every Linear of the transformer), IMAGE_GUIDANCE (default 1: generate's
+image_guidance_scale; other values add the uncond forward to every step, with U_i = the condition latents), STEPS.
+Prints the card name and power limit with the timing."""
 import os, sys, json, subprocess, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,6 +23,7 @@ latent_lora = os.environ.get("LATENT_LORA", "0") == "1"
 lora_rank = int(os.environ.get("LORA_RANK", "32"))
 lora_scale = float(os.environ.get("LORA_SCALE", "1"))
 lora_targets = os.environ.get("LORA_TARGETS", "config")
+image_guidance = float(os.environ.get("IMAGE_GUIDANCE", "1"))
 model_config = {"union_cond_attn": True, "latent_lora": latent_lora}
 jak = {"scale": lora_scale} if lora_scale != 1.0 else None
 pipe = B200FluxPipeline.from_synthetic(cfg, seed=0, device=dev, lora_rank=lora_rank if use_lora else 0)
@@ -36,6 +38,7 @@ cond = Condition("cot", latents=torch.randn(1, 1024, 64, generator=g).to(torch.b
 K = int(os.environ.get("STEPS", "8"))
 def run(n):
     return generate(pipe, conditions=[cond], model_config=model_config, default_lora=True, joint_attention_kwargs=jak,
+                    image_guidance_scale=image_guidance,
                     prompt_embeds=txt, pooled_prompt_embeds=pool, latents=lat, height=1024, width=1024,
                     num_inference_steps=n, output_type="latent").images
 run(3); torch.cuda.synchronize()
@@ -50,6 +53,7 @@ except Exception:
     power_limit = "unknown"
 print(json.dumps({"entry": "B", "lora": use_lora, "lora_mode": pipe.transformer.lora_mode, "latent_lora": latent_lora,
                   "lora_rank": lora_rank if use_lora else 0, "lora_scale": lora_scale, "lora_targets": lora_targets,
+                  "image_guidance_scale": image_guidance,
                   "n_tok": 5632, "ms_per_step": ms, "steps_per_s": 1e3 / ms, "step_tflop": tf, "tflops": tf / ms * 1e3,
                   "finite": bool(torch.isfinite(out.float()).all()), "gpu": torch.cuda.get_device_name(dev),
                   "power_limit": power_limit}))
