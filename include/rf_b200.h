@@ -292,11 +292,13 @@ void rf_text_destroy(rf_text* h);
 int rf_text_load_weight(rf_text* h, const char* key, const void* src, int64_t numel);
 /* number of keys under `prefix` ("t5." / "clip.") not loaded yet (names in rf_last_error) */
 int rf_text_missing_weights(rf_text* h, const char* prefix);
-/* ids: device int32 [batch, seq]; position_bias: device bf16 [heads, seq, seq] (layer-0 relative
+/* ids: device int32 [batch, seq], every id in [0, t5_vocab) (not checked on the device: an id outside reads
+ * outside the embedding table); position_bias: device bf16 [heads, seq, seq] (layer-0 relative
  * attention bias, shared by all layers; bucketed on the host); out: device bf16 [batch, seq, d_model] */
 int rf_t5_encode(rf_text* h, const int* ids, int batch, int seq, const void* position_bias, void* out,
                  void* stream);
-/* ids: device int32 [batch, seq <= 77]; eos_pos: device int32 [batch] (pooling position, = ids.argmax(-1)
+/* ids: device int32 [batch, seq <= 77], every id in [0, clip_vocab) (not checked on the device, as for
+ * rf_t5_encode); eos_pos: device int32 [batch] in [0, seq) (pooling position, = ids.argmax(-1)
  * for the stock CLIP-L config); pooled_out bf16 [batch, d_model]; hidden_out (nullable) bf16 [batch, seq, d_model] */
 int rf_clip_encode(rf_text* h, const int* ids, const int* eos_pos, int batch, int seq, void* pooled_out,
                    void* hidden_out, void* stream);

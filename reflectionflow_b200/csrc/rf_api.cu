@@ -168,6 +168,38 @@ int rf_dbg_text_attention(const void* q, const void* k, const void* v, int ld, v
                                  use_scale, causal, static_cast<cudaStream_t>(stream));
 }
 
+// Test hooks over the text encoders' launchers (csrc/text.cu): the same host code rf_t5_encode / rf_clip_encode run,
+// on caller-owned buffers.  Layouts: rf_internal.h.
+int rf_dbg_text_embed(const int* ids, const void* table, const void* pos, void* out, int T, int S, int D,
+                      void* stream) {
+  return rf::text_embed_launch(ids, static_cast<const bf16*>(table), static_cast<const bf16*>(pos),
+                               static_cast<bf16*>(out), T, S, D, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_text_rownorm(const void* x, void* out, int rows, int dim, const void* w, const void* b, float eps, int mode,
+                        void* stream) {
+  return rf::text_rownorm_launch(static_cast<const bf16*>(x), static_cast<bf16*>(out), rows, dim,
+                                 static_cast<const bf16*>(w), static_cast<const bf16*>(b), eps, mode,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_text_ewise(const void* a, const void* b, void* out, int64_t n, int mode, void* stream) {
+  return rf::text_ewise_launch(static_cast<const bf16*>(a), static_cast<const bf16*>(b), static_cast<bf16*>(out), n,
+                               mode, static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_text_gather_rows(const void* x, const int* pos, void* out, int B, int S, int D, void* stream) {
+  return rf::text_gather_rows_launch(static_cast<const bf16*>(x), pos, static_cast<bf16*>(out), B, S, D,
+                                     static_cast<cudaStream_t>(stream));
+}
+
+int rf_dbg_t5_gated_gelu(const void* x, int T, int D, const void* wi0, const void* wi1, int F, void* h0, void* h1,
+                         void* stream) {
+  return rf::t5_gated_gelu(static_cast<const bf16*>(x), T, D, static_cast<const bf16*>(wi0),
+                           static_cast<const bf16*>(wi1), F, static_cast<bf16*>(h0), static_cast<bf16*>(h1),
+                           static_cast<cudaStream_t>(stream));
+}
+
 // Test hooks over the VAE's launchers (csrc/vae.cu, the convolution in csrc/gemm_sm90.cu): the same host code
 // rf_vae_decode / rf_vae_encode run, on caller-owned buffers.  Layouts: rf_internal.h.
 int rf_dbg_vae_conv(const void* in, const void* weight, const void* bias, void* out, const void* res, const void* ones,

@@ -140,6 +140,25 @@ bool text_attn_tc_eligible(int S, int ld, int ldo);
 int text_attn_tc_launch(const bf16* q, const bf16* k, const bf16* v, int ld, bf16* out, int ldo, int B, int S,
                         int heads, const bf16* bias, float scale, int use_scale, int causal, cudaStream_t stream);
 
+// The text encoders' own kernels (text.cu), the launchers rf_t5_encode / rf_clip_encode call.  Rows are bf16,
+// 16-byte aligned, with widths that are multiples of 8.
+// out[t, :] = table[ids[t], :], or bf16(table[ids[t], :] + pos[t % S, :]) with pos; ids must lie in the table
+int text_embed_launch(const int* ids, const bf16* table, const bf16* pos, bf16* out, int T, int S, int D,
+                      cudaStream_t stream);
+// mode 0, T5LayerNorm:  out = bf16(w * bf16(x / sqrt(mean(x^2) + eps)))
+// mode 1, LayerNorm:    out = bf16((x - mean) / sqrt(var + eps) * w + b)           (fp32 statistics, two passes)
+int text_rownorm_launch(const bf16* x, bf16* out, int rows, int dim, const bf16* w, const bf16* b, float eps,
+                        int mode, cudaStream_t stream);
+// n elements (n % 8 == 0), out may alias a.  mode 0: out = bf16(gelu_new(a) * b), transformers' NewGELUActivation
+// with eager bf16's rounding after every op; mode 1: out = bf16(a * bf16(sigmoid(bf16(1.702 a)))) (quick_gelu)
+int text_ewise_launch(const bf16* a, const bf16* b, bf16* out, int64_t n, int mode, cudaStream_t stream);
+// out[b, :] = x[b * S + pos[b], :] for b < B (x: [B * S, D])
+int text_gather_rows_launch(const bf16* x, const int* pos, bf16* out, int B, int S, int D, cudaStream_t stream);
+// T5's gated feed-forward up to wo on x [T, D]: h0 = bf16(x wi0^T), h1 = bf16(x wi1^T) (wi: [F, D]), then
+// h0 = bf16(gelu_new(h0) * h1) in place.  h0, h1: [T, F]
+int t5_gated_gelu(const bf16* x, int T, int D, const bf16* wi0, const bf16* wi1, int F, bf16* h0, bf16* h1,
+                  cudaStream_t stream);
+
 // ---------------------------------------------------------------------------- bandwidth kernels
 // out = bf16(bf16(bf16(LN(x)) * bf16(1 + scale)) + shift)   (LN: no affine, eps 1e-6)
 //   rows of batch element b (= row / rows_per_batch) use scale/shift + b * mod_stride

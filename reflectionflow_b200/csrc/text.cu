@@ -6,7 +6,7 @@
 // pipeline_tools.py:33-52) — each reflection candidate has its own refined prompt
 // (tts/tts_reflectionflow.py:286-294).  Token ids in (tokenizers stay on the host), embeddings out.
 //
-// All Linear layers run on the wgmma GEMM kernel of this library (fused residual / GELU
+// All Linear layers run on the wgmma GEMM kernel of this library (fused bias / residual
 // epilogues); the pieces specific to the text encoders are small bandwidth kernels here: T5 RMSNorm,
 // affine LayerNorm, embedding gathers, the gated-GELU product, quick-GELU, and a shared-memory
 // attention for short sequences with head_dim 64 (T5: additive relative-position bias, no scaling;
@@ -129,7 +129,21 @@ rownorm_kernel(const bf16* __restrict__ x, bf16* __restrict__ out, int rows, int
   }
 }
 
-// out = bf16(a * b)  (gated-GELU product)   |  mode 1: out = bf16(a * sigmoid(1.702 a)) (quick_gelu)
+// transformers' NewGELUActivation ("gelu_new", T5-v1.1's dense_act_fn) as eager bf16 torch evaluates
+// 0.5 * x * (1 + tanh(sqrt(2/pi) * (x + 0.044715 * pow(x, 3)))): every op rounds to bf16, pow(x, 3) as (x * x) * x.
+// (The DiT's EPI_GELU is diffusers' GELU(approximate="tanh"), one fused op with a single rounding: not this.)
+__device__ __forceinline__ float gelu_new_bf16(float x) {
+  const float p = bf16_round(__fmul_rn(bf16_round(__fmul_rn(x, x)), x));
+  const float q = bf16_round(__fmul_rn(0.044715f, p));
+  const float r = bf16_round(__fadd_rn(x, q));
+  const float s = bf16_round(__fmul_rn(0.7978845608f, r));
+  const float t = bf16_round(tanhf(s));
+  const float u = bf16_round(__fadd_rn(1.0f, t));
+  const float h = bf16_round(__fmul_rn(0.5f, x));
+  return bf16_round(__fmul_rn(h, u));
+}
+
+// out = bf16(gelu_new(a) * b)  (T5's gated-GELU product)   |  mode 1: out = bf16(a * sigmoid(1.702 a)) (quick_gelu)
 // (a and out may alias: every thread reads its 8 elements before writing them)
 __global__ void ewise_kernel(const bf16* a, const bf16* b, bf16* out, long long n8, int mode) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -143,7 +157,7 @@ __global__ void ewise_kernel(const bf16* a, const bf16* b, bf16* out, long long 
   for (int k = 0; k < 4; ++k) {
     const float2 x = unpack_bf16x2(xs[k]), y = unpack_bf16x2(ys[k]);
     if (mode == 0) {
-      o[k] = pack_bf16x2(x.x * y.x, x.y * y.y);
+      o[k] = pack_bf16x2(__fmul_rn(gelu_new_bf16(x.x), y.x), __fmul_rn(gelu_new_bf16(x.y), y.y));
     } else {  // x * sigmoid(1.702 x): torch evaluates sigmoid(bf16(1.702 x)) in fp32 and rounds, then multiplies
       const float s0 = bf16_round(1.0f / (1.0f + expf(-bf16_round(1.702f * x.x))));
       const float s1 = bf16_round(1.0f / (1.0f + expf(-bf16_round(1.702f * x.y))));
@@ -285,6 +299,54 @@ __global__ void gather_rows_kernel(const bf16* __restrict__ x, const int* __rest
   for (int i = threadIdx.x; i < D; i += blockDim.x) out[static_cast<size_t>(b) * D + i] = src[i];
 }
 
+// ---- launchers: the encoders below and the rf_dbg_text_* test hooks (rf_api.cu) both go through these
+int text_embed_launch(const int* ids, const bf16* table, const bf16* pos, bf16* out, int T, int S, int D,
+                      cudaStream_t s) {
+  if (T <= 0 || S <= 0 || D % 8) {
+    set_error("text_embed: needs T, S > 0 and D % 8 == 0");
+    return -1;
+  }
+  embed_kernel<<<T, 128, 0, s>>>(ids, table, pos, out, T, S, D);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int text_rownorm_launch(const bf16* x, bf16* out, int rows, int dim, const bf16* w, const bf16* b, float eps,
+                        int mode, cudaStream_t s) {
+  if (rows <= 0 || dim <= 0 || dim % 8 || (mode != 0 && mode != 1) || (mode == 1 && !b)) {
+    set_error("text_rownorm: needs rows > 0, dim % 8 == 0, mode 0 or 1 (mode 1 with a bias)");
+    return -1;
+  }
+  rownorm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, out, rows, dim, w, b, eps, mode);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int text_ewise_launch(const bf16* a, const bf16* b, bf16* out, int64_t n, int mode, cudaStream_t s) {
+  if (n <= 0 || n % 8 || (mode != 0 && mode != 1) || (mode == 0 && !b)) {
+    set_error("text_ewise: needs n > 0, n % 8 == 0, mode 0 (with b) or 1");
+    return -1;
+  }
+  const long long n8 = n / 8;
+  ewise_kernel<<<static_cast<int>((n8 + 255) / 256), 256, 0, s>>>(a, b, out, n8, mode);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+int text_gather_rows_launch(const bf16* x, const int* pos, bf16* out, int B, int S, int D, cudaStream_t s) {
+  if (B <= 0 || S <= 0 || D <= 0) {
+    set_error("text_gather_rows: empty problem");
+    return -1;
+  }
+  gather_rows_kernel<<<B, 128, 0, s>>>(x, pos, out, S, D);
+  RF_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
 }  // namespace rf
 
 using rf::bf16;
@@ -333,13 +395,6 @@ bf16* take(rf_text* h, int64_t n, int& rc, const std::string& key = "") {
 // a slice of a packed matrix registered under its own key
 void alias(rf_text* h, const std::string& key, bf16* p, int64_t n) { h->slots[key] = {p, n, false}; }
 
-int rownorm(const bf16* x, bf16* out, int rows, int dim, const bf16* w, const bf16* b, float eps, int mode,
-            cudaStream_t s) {
-  rf::rownorm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, out, rows, dim, w, b, eps, mode);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
-  return 0;
-}
 int linear(int epi, const bf16* A, int lda, int M, const bf16* W, const bf16* bias, bf16* out, int ldo, int N,
            int K, const bf16* res, int ldr, const bf16* ones, cudaStream_t s) {
   rf::GemmGroupArgs g;
@@ -403,6 +458,16 @@ int missing(rf_text* h, const char* prefix) {
   return n;
 }
 }  // namespace
+
+namespace rf {
+// T5DenseGatedActDense up to wo: h0 = bf16(x wi_0^T), h1 = bf16(x wi_1^T), h0 = bf16(gelu_new(h0) * h1)
+int t5_gated_gelu(const bf16* x, int T, int D, const bf16* wi0, const bf16* wi1, int F, bf16* h0, bf16* h1,
+                  cudaStream_t s) {
+  RF_TRYT(linear(EPI_BIAS, x, D, T, wi0, nullptr, h0, F, F, D, nullptr, 0, nullptr, s));
+  RF_TRYT(linear(EPI_BIAS, x, D, T, wi1, nullptr, h1, F, F, D, nullptr, 0, nullptr, s));
+  return text_ewise_launch(h0, h1, h0, static_cast<int64_t>(T) * F, 0, s);
+}
+}  // namespace rf
 
 extern "C" {
 
@@ -522,26 +587,19 @@ int rf_t5_encode(rf_text* h, const int* ids, int batch, int seq, const void* pos
   const int D = c.t5_d_model, F = c.t5_d_ff, I = c.t5_heads * 64, T = batch * seq;
   RF_TRYT(ensure_ws(h, T));
   bf16* xo = static_cast<bf16*>(out);  // residual stream lives in the caller's output buffer
-  rf::embed_kernel<<<T, 128, 0, s>>>(ids, h->t5_shared, nullptr, xo, T, seq, D);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYT(rf::text_embed_launch(ids, h->t5_shared, nullptr, xo, T, seq, D, s));
   for (int i = 0; i < c.t5_layers; ++i) {
     const T5Layer& L = h->t5[i];
-    RF_TRYT(rownorm(xo, h->xn, T, D, L.ln0, nullptr, c.t5_eps, 0, s));
+    RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln0, nullptr, c.t5_eps, 0, s));
     RF_TRYT(linear(rf::EPI_BIAS, h->xn, D, T, L.qkv, nullptr, h->qkv, 3 * I, 3 * I, D, nullptr, 0, nullptr, s));
     RF_TRYT(small_attn(h->qkv, h->qkv + I, h->qkv + 2 * I, 3 * I, h->att, I, batch, seq, c.t5_heads,
                        static_cast<const bf16*>(position_bias), 1.0f, 0, 0, s));
     RF_TRYT(linear(rf::EPI_GATE_RES, h->att, I, T, L.o, nullptr, xo, D, D, I, xo, D, h->ones, s));
-    RF_TRYT(rownorm(xo, h->xn, T, D, L.ln1, nullptr, c.t5_eps, 0, s));
-    RF_TRYT(linear(rf::EPI_GELU, h->xn, D, T, L.wi0, nullptr, h->h0, F, F, D, nullptr, 0, nullptr, s));
-    RF_TRYT(linear(rf::EPI_BIAS, h->xn, D, T, L.wi1, nullptr, h->h1, F, F, D, nullptr, 0, nullptr, s));
-    const long long n8 = static_cast<long long>(T) * F / 8;
-    rf::ewise_kernel<<<static_cast<int>((n8 + 255) / 256), 256, 0, s>>>(h->h0, h->h1, h->h0, n8, 0);
-    RF_CHECK_CUDA(cudaGetLastError());
-    rf::count_launch();
+    RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln1, nullptr, c.t5_eps, 0, s));
+    RF_TRYT(rf::t5_gated_gelu(h->xn, T, D, L.wi0, L.wi1, F, h->h0, h->h1, s));
     RF_TRYT(linear(rf::EPI_GATE_RES, h->h0, F, T, L.wo, nullptr, xo, D, D, F, xo, D, h->ones, s));
   }
-  RF_TRYT(rownorm(xo, h->xn, T, D, h->t5_final, nullptr, c.t5_eps, 0, s));
+  RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, h->t5_final, nullptr, c.t5_eps, 0, s));
   RF_CHECK_CUDA(cudaMemcpyAsync(xo, h->xn, static_cast<size_t>(T) * D * 2, cudaMemcpyDeviceToDevice, s));
   return 0;
 }
@@ -558,31 +616,23 @@ int rf_clip_encode(rf_text* h, const int* ids, const int* eos_pos, int batch, in
   const int C = c.clip_d_model, T = batch * seq;
   RF_TRYT(ensure_ws(h, T));
   bf16* x = h->x;
-  rf::embed_kernel<<<T, 128, 0, s>>>(ids, h->clip_tok, h->clip_pos, x, T, seq, C);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
+  RF_TRYT(rf::text_embed_launch(ids, h->clip_tok, h->clip_pos, x, T, seq, C, s));
   for (int i = 0; i < c.clip_layers; ++i) {
     const ClipLayer& L = h->clip[i];
-    RF_TRYT(rownorm(x, h->xn, T, C, L.ln1w, L.ln1b, 1e-5f, 1, s));
+    RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, L.ln1w, L.ln1b, 1e-5f, 1, s));
     RF_TRYT(linear(rf::EPI_BIAS, h->xn, C, T, L.qkvw, L.qkvb, h->qkv, 3 * C, 3 * C, C, nullptr, 0, nullptr, s));
     RF_TRYT(small_attn(h->qkv, h->qkv + C, h->qkv + 2 * C, 3 * C, h->att, C, batch, seq, c.clip_heads, nullptr,
                        0.125f, 1, 1, s));
     RF_TRYT(linear(rf::EPI_GATE_RES, h->att, C, T, L.ow, L.ob, x, C, C, C, x, C, h->ones, s));
-    RF_TRYT(rownorm(x, h->xn, T, C, L.ln2w, L.ln2b, 1e-5f, 1, s));
+    RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, L.ln2w, L.ln2b, 1e-5f, 1, s));
     RF_TRYT(linear(rf::EPI_BIAS, h->xn, C, T, L.fc1w, L.fc1b, h->h0, 4 * C, 4 * C, C, nullptr, 0, nullptr, s));
-    const long long n8 = static_cast<long long>(T) * 4 * C / 8;
-    rf::ewise_kernel<<<static_cast<int>((n8 + 255) / 256), 256, 0, s>>>(h->h0, nullptr, h->h0, n8, 1);
-    RF_CHECK_CUDA(cudaGetLastError());
-    rf::count_launch();
+    RF_TRYT(rf::text_ewise_launch(h->h0, nullptr, h->h0, static_cast<int64_t>(T) * 4 * C, 1, s));
     RF_TRYT(linear(rf::EPI_GATE_RES, h->h0, 4 * C, T, L.fc2w, L.fc2b, x, C, C, 4 * C, x, C, h->ones, s));
   }
-  RF_TRYT(rownorm(x, h->xn, T, C, h->clip_fw, h->clip_fb, 1e-5f, 1, s));
+  RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, h->clip_fw, h->clip_fb, 1e-5f, 1, s));
   if (hidden_out)
     RF_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h->xn, static_cast<size_t>(T) * C * 2, cudaMemcpyDeviceToDevice, s));
-  rf::gather_rows_kernel<<<batch, 128, 0, s>>>(h->xn, eos_pos, static_cast<bf16*>(pooled_out), seq, C);
-  RF_CHECK_CUDA(cudaGetLastError());
-  rf::count_launch();
-  return 0;
+  return rf::text_gather_rows_launch(h->xn, eos_pos, static_cast<bf16*>(pooled_out), batch, seq, C, s);
 }
 
 }  // extern "C"

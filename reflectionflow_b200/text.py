@@ -180,8 +180,17 @@ class B200TextEncoders:
             self._bias[seq] = self._rel_bias[idx].permute(2, 0, 1).contiguous()
         return self._bias[seq]
 
+    @staticmethod
+    def _check_ids(input_ids: torch.Tensor, vocab: int, what: str):
+        """the embedding kernel indexes its table with the ids unchecked: refuse an id outside [0, vocab) before any
+        launch (on the caller's tensor, before the copy to the device)"""
+        if input_ids.numel() and (int(input_ids.min()) < 0 or int(input_ids.max()) >= vocab):
+            raise L.RFError(f"{what}: token id outside [0, {vocab}) (min {int(input_ids.min())}, "
+                            f"max {int(input_ids.max())})")
+
     def t5_encode(self, input_ids: torch.Tensor) -> torch.Tensor:
         """ids [B, S] -> last_hidden_state [B, S, d_model] bf16 (no attention mask: FLUX passes none)"""
+        self._check_ids(input_ids, self.cfg["t5_vocab"], "t5_encode")
         ids = input_ids.to(self.device, torch.int32).contiguous()
         B, S = ids.shape
         out = torch.empty(B, S, self.cfg["t5_d_model"], device=self.device, dtype=torch.bfloat16)
@@ -196,6 +205,7 @@ class B200TextEncoders:
         """ids [B, S<=77] -> pooler_output [B, d] (hidden state at the EOS position), optionally
         last_hidden_state.  eos_token_id == 2 is the stock CLIP-L config, for which transformers
         pools at ids.argmax(-1); otherwise at the first occurrence of eos_token_id."""
+        self._check_ids(input_ids, self.cfg["clip_vocab"], "clip_encode")
         ids = input_ids.to(self.device, torch.int32).contiguous()
         B, S = ids.shape
         if eos_token_id == 2:

@@ -3,7 +3,8 @@
 The reference gets its text embeddings from diffusers FluxPipeline.encode_prompt, i.e. from the
 transformers classes (train_flux/flux/generate.py:148-161) — transformers is installed in this image,
 so it is imported directly as the oracle (CPU, eager attention, bf16 like the reference loads it, and
-fp32 as the "true value").  Floating-point bar, as for the DiT (DESIGN.md §5): our error against the
+fp32 as the "true value"; the bf16 model also runs on the device, where the reference runs it, and
+the distance to it is printed).  Floating-point bar, as for the DiT (DESIGN.md §5): our error against the
 fp32 model may not exceed 1.25x the error of the reference's own bf16 arithmetic against it, and the
 two bf16 results agree to a few 1e-3 of the mean magnitude."""
 import pytest
@@ -15,6 +16,18 @@ pytestmark = pytest.mark.gpu
 def _rel(a, b):
     a, b = a.float().cpu(), b.float().cpu()
     return ((a - b).abs().mean() / b.abs().mean()).item()
+
+
+def _vs_cuda_bf16(m16, ids, ours, pick):
+    """the bf16 transformers model run on the device, where the reference runs it: (mean error of ours against it
+    relative to its mean magnitude, fraction of bit-identical elements)"""
+    import copy
+    mc = copy.deepcopy(m16).to("cuda")
+    with torch.no_grad():
+        ref = pick(mc(input_ids=ids.to("cuda"))).reshape(ours.shape)
+    same = (ours.view(torch.int16) == ref.view(torch.int16)).float().mean().item()
+    del mc
+    return _rel(ours, ref), same
 
 
 def _t5_models(layers, d_model, d_ff, heads, vocab, seed):
@@ -63,7 +76,9 @@ def test_t5_encoder_matches_transformers(layers, d_model, d_ff, heads, B, S):
     torch.cuda.synchronize()
     assert out.shape == ref16.shape and out.dtype == torch.bfloat16
     e_ref, e_ours, e_pair = _rel(ref16, ref32), _rel(out, ref32), _rel(out, ref16)
-    print(f"t5 L{layers} d{d_model} S{S}: ref-bf16 vs fp32 {e_ref:.3e}, ours vs fp32 {e_ours:.3e}, ours vs ref-bf16 {e_pair:.3e}")
+    e_cuda, same = _vs_cuda_bf16(m16, ids, out, lambda r: r[0])
+    print(f"t5 L{layers} d{d_model} S{S}: ref-bf16 vs fp32 {e_ref:.3e}, ours vs fp32 {e_ours:.3e}, ours vs ref-bf16 {e_pair:.3e}, "
+          f"ours vs CUDA bf16 {e_cuda:.3e} (bit-identical {same:.4f})")
     assert e_ours <= 1.25 * e_ref + 1e-4
     assert e_pair <= 2.0 * e_ref + 1e-4      # two independent bf16 roundings of the same fp32 function
 
@@ -122,7 +137,9 @@ def test_clip_text_model_matches_transformers(layers, B, S):
     torch.cuda.synchronize()
     e_ref, e_ours = _rel(r16.last_hidden_state, r32.last_hidden_state), _rel(hidden, r32.last_hidden_state)
     p_ref, p_ours = _rel(r16.pooler_output, r32.pooler_output), _rel(pooled, r32.pooler_output)
-    print(f"clip L{layers} S{S}: hidden ref {e_ref:.3e} ours {e_ours:.3e}; pooled ref {p_ref:.3e} ours {p_ours:.3e}")
+    e_cuda, same = _vs_cuda_bf16(m16, ids, hidden, lambda r: r.last_hidden_state)
+    print(f"clip L{layers} S{S}: hidden ref {e_ref:.3e} ours {e_ours:.3e}; pooled ref {p_ref:.3e} ours {p_ours:.3e}; "
+          f"hidden ours vs CUDA bf16 {e_cuda:.3e} (bit-identical {same:.4f})")
     assert e_ours <= 1.25 * e_ref + 1e-4
     assert p_ours <= 1.5 * p_ref + 1e-4       # B x 768 values only: noisier statistic
     # pooled is the hidden state at the EOS position, bit for bit
