@@ -39,21 +39,9 @@ int gemv_init();
 
 using rf::bf16;
 
-#define RF_TRY(expr)            \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != 0) return _rc;   \
-  } while (0)
-
 namespace {
 
-struct Slot {
-  bf16* dst;
-  int64_t numel;
-  bool loaded;
-};
-
-struct Lin {  // views into the weight arena
+struct Lin {  // a Linear's weights, or views into a packed one
   bf16* w = nullptr;
   bf16* b = nullptr;
 };
@@ -111,9 +99,9 @@ struct rf_dit {
   int D = 0;
   int device = 0;
   // ---- weights
-  std::vector<void*> allocs;      // weights: live until destroy
-  std::vector<void*> geo_allocs;  // workspace of the current geometry: freed on re-prepare
-  std::unordered_map<std::string, Slot> slots;
+  rf::DeviceAllocs mem;      // weights, LoRA factors, merged copies: live until destroy
+  rf::DeviceAllocs geo_mem;  // workspace of the current geometry: freed on re-prepare
+  rf::WeightTable weights;
   std::unordered_map<std::string, LoraT*> lora_slots;
   Lin x_emb, ctx_emb, t1, t2, g1, g2, p1, p2, proj_out;
   LoraPack l_x_emb;
@@ -162,8 +150,7 @@ struct rf_dit {
   float* s_igs = nullptr;
   int s_cap_steps_u = 0;
   StepGraph graph, graph_ig;  // the captured step of rf_dit_denoise / of the guided loop
-  cudaStream_t own_stream = nullptr;  // capture is illegal on the legacy default stream
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+  rf::SideStream side;        // the denoise loop's stream
 };
 
 namespace {
@@ -173,62 +160,44 @@ float lora_eff(const rf_dit* h, const LoraT& t) { return static_cast<float>(t.sc
 // a target whose effective scaling is 0 adds exactly nothing: it runs no launch at all
 bool lora_on(const rf_dit* h, const LoraT& t) { return t.set && lora_eff(h, t) != 0.f; }
 
-int dev_alloc(rf_dit* h, void** p, size_t bytes, bool geometry = false) {
-  RF_CHECK_CUDA(cudaMalloc(p, bytes ? bytes : 16));
-  (geometry ? h->geo_allocs : h->allocs).push_back(*p);
+// Linear whose weight/bias may be a row range of a packed matrix
+void reg_lin(rf_dit* h, const std::string& mod, bf16* w, bf16* b, int out, int in) {
+  h->weights.add(mod + ".weight", w, static_cast<int64_t>(out) * in);
+  h->weights.add(mod + ".bias", b, out);
+}
+
+// a Linear's own storage, registered under `mod` (empty: a packed one whose row ranges the caller registers)
+int new_lin(rf_dit* h, Lin& l, const std::string& mod, int out, int in) {
+  RF_TRY(h->mem.alloc(&l.w, static_cast<size_t>(out) * in));
+  RF_TRY(h->mem.alloc(&l.b, out));
+  if (!mod.empty()) reg_lin(h, mod, l.w, l.b, out, in);
   return 0;
 }
 
-struct Arena {
-  rf_dit* h;
-  int fail = 0;
-  bf16* take(int64_t numel) {
-    void* p = nullptr;
-    if (dev_alloc(h, &p, static_cast<size_t>(numel) * 2)) fail = -2;
-    return static_cast<bf16*>(p);
-  }
-};
-
-void reg(rf_dit* h, const std::string& key, bf16* dst, int64_t numel) {
-  h->slots[key] = Slot{dst, numel, false};
-}
-
-// Linear whose weight/bias may be a row range of a packed matrix
-void reg_lin(rf_dit* h, const std::string& mod, bf16* w, bf16* b, int out, int in) {
-  reg(h, mod + ".weight", w, static_cast<int64_t>(out) * in);
-  reg(h, mod + ".bias", b, out);
-}
-
-Lin new_lin(rf_dit* h, Arena& ar, const std::string& mod, int out, int in) {
-  Lin l;
-  l.w = ar.take(static_cast<int64_t>(out) * in);
-  l.b = ar.take(out);
-  if (!mod.empty()) reg_lin(h, mod, l.w, l.b, out, in);
-  return l;
+// a weight vector's own storage, registered under `key`
+int new_vec(rf_dit* h, bf16** v, const std::string& key, int n) {
+  RF_TRY(h->mem.alloc(v, n));
+  h->weights.add(key, *v, n);
+  return 0;
 }
 
 // Zeroed factor storage of pack p, live until destroy: unset members must add exactly nothing (a q-only adapter
 // still runs the stacked q|k|v path).  A preset A is a view into a larger stack and is only zeroed.
 int lora_storage(rf_dit* h, LoraPack& p) {
   if (p.B != nullptr) return 0;
-  const size_t a = static_cast<size_t>(p.n) * h->lora_pad * p.t[0].in * 2;
-  const size_t b = static_cast<size_t>(p.n) * p.t[0].out * h->lora_pad * 2;
-  void* q = nullptr;
-  if (p.A == nullptr) {
-    RF_TRY(dev_alloc(h, &q, a));
-    p.A = static_cast<bf16*>(q);
-  }
-  RF_TRY(dev_alloc(h, &q, b));
-  p.B = static_cast<bf16*>(q);
-  RF_CHECK_CUDA(cudaMemset(p.A, 0, a));
-  RF_CHECK_CUDA(cudaMemset(p.B, 0, b));
+  const size_t a = static_cast<size_t>(p.n) * h->lora_pad * p.t[0].in;
+  const size_t b = static_cast<size_t>(p.n) * p.t[0].out * h->lora_pad;
+  if (p.A == nullptr) RF_TRY(h->mem.alloc(&p.A, a));
+  RF_TRY(h->mem.alloc(&p.B, b));
+  RF_CHECK_CUDA(cudaMemset(p.A, 0, a * 2));
+  RF_CHECK_CUDA(cudaMemset(p.B, 0, b * 2));
   return 0;
 }
 
 // the pack of the targets `mods`, each out x in and stacked in that order; W: the packed projection weight
-void new_pack(rf_dit* h, Arena& ar, LoraPack& p, std::initializer_list<std::string> mods, int out, int in,
-              const bf16* W, bool always) {
-  if (h->cfg.lora_rank <= 0) return;
+int new_pack(rf_dit* h, LoraPack& p, std::initializer_list<std::string> mods, int out, int in, const bf16* W,
+             bool always) {
+  if (h->cfg.lora_rank <= 0) return 0;
   for (const std::string& m : mods) {
     p.t[p.n] = LoraT{in, out, false, 1.0, &p, p.n};
     h->lora_slots[m] = &p.t[p.n++];
@@ -236,39 +205,38 @@ void new_pack(rf_dit* h, Arena& ar, LoraPack& p, std::initializer_list<std::stri
   p.always = always;
   p.W = W;
   if (W) h->proj_packs.push_back(&p);
-  if (!always && lora_storage(h, p)) ar.fail = -2;
+  return always ? 0 : lora_storage(h, p);
 }
 
 int build_storage(rf_dit* h) {
   const rf_dit_config& c = h->cfg;
   const int D = h->D, lpad = h->lora_pad;
-  Arena ar{h};
-  h->x_emb = new_lin(h, ar, "x_embedder", D, c.in_channels);
-  new_pack(h, ar, h->l_x_emb, {"x_embedder"}, D, c.in_channels, h->x_emb.w, false);
-  h->ctx_emb = new_lin(h, ar, "context_embedder", D, c.joint_attention_dim);
-  new_pack(h, ar, h->l_ctx, {"context_embedder"}, D, c.joint_attention_dim, h->ctx_emb.w, true);
+  RF_TRY(new_lin(h, h->x_emb, "x_embedder", D, c.in_channels));
+  RF_TRY(new_pack(h, h->l_x_emb, {"x_embedder"}, D, c.in_channels, h->x_emb.w, false));
+  RF_TRY(new_lin(h, h->ctx_emb, "context_embedder", D, c.joint_attention_dim));
+  RF_TRY(new_pack(h, h->l_ctx, {"context_embedder"}, D, c.joint_attention_dim, h->ctx_emb.w, true));
   const std::string tte = "time_text_embed.";
-  h->t1 = new_lin(h, ar, tte + "timestep_embedder.linear_1", D, 256);
-  h->t2 = new_lin(h, ar, tte + "timestep_embedder.linear_2", D, D);
-  new_pack(h, ar, h->l_t1, {tte + "timestep_embedder.linear_1"}, D, 256, nullptr, true);
-  new_pack(h, ar, h->l_t2, {tte + "timestep_embedder.linear_2"}, D, D, nullptr, true);
+  RF_TRY(new_lin(h, h->t1, tte + "timestep_embedder.linear_1", D, 256));
+  RF_TRY(new_lin(h, h->t2, tte + "timestep_embedder.linear_2", D, D));
+  RF_TRY(new_pack(h, h->l_t1, {tte + "timestep_embedder.linear_1"}, D, 256, nullptr, true));
+  RF_TRY(new_pack(h, h->l_t2, {tte + "timestep_embedder.linear_2"}, D, D, nullptr, true));
   if (c.guidance_embeds) {
-    h->g1 = new_lin(h, ar, tte + "guidance_embedder.linear_1", D, 256);
-    h->g2 = new_lin(h, ar, tte + "guidance_embedder.linear_2", D, D);
-    new_pack(h, ar, h->l_g1, {tte + "guidance_embedder.linear_1"}, D, 256, nullptr, true);
-    new_pack(h, ar, h->l_g2, {tte + "guidance_embedder.linear_2"}, D, D, nullptr, true);
+    RF_TRY(new_lin(h, h->g1, tte + "guidance_embedder.linear_1", D, 256));
+    RF_TRY(new_lin(h, h->g2, tte + "guidance_embedder.linear_2", D, D));
+    RF_TRY(new_pack(h, h->l_g1, {tte + "guidance_embedder.linear_1"}, D, 256, nullptr, true));
+    RF_TRY(new_pack(h, h->l_g2, {tte + "guidance_embedder.linear_2"}, D, D, nullptr, true));
   }
-  h->p1 = new_lin(h, ar, tte + "text_embedder.linear_1", D, c.pooled_projection_dim);
-  h->p2 = new_lin(h, ar, tte + "text_embedder.linear_2", D, D);
-  new_pack(h, ar, h->l_p1, {tte + "text_embedder.linear_1"}, D, c.pooled_projection_dim, nullptr, true);
-  new_pack(h, ar, h->l_p2, {tte + "text_embedder.linear_2"}, D, D, nullptr, true);
-  h->proj_out = new_lin(h, ar, "proj_out", c.in_channels, D);
-  new_pack(h, ar, h->l_proj_out, {"proj_out"}, c.in_channels, D, h->proj_out.w, true);
+  RF_TRY(new_lin(h, h->p1, tte + "text_embedder.linear_1", D, c.pooled_projection_dim));
+  RF_TRY(new_lin(h, h->p2, tte + "text_embedder.linear_2", D, D));
+  RF_TRY(new_pack(h, h->l_p1, {tte + "text_embedder.linear_1"}, D, c.pooled_projection_dim, nullptr, true));
+  RF_TRY(new_pack(h, h->l_p2, {tte + "text_embedder.linear_2"}, D, D, nullptr, true));
+  RF_TRY(new_lin(h, h->proj_out, "proj_out", c.in_channels, D));
+  RF_TRY(new_pack(h, h->l_proj_out, {"proj_out"}, c.in_channels, D, h->proj_out.w, true));
 
   h->n_mod = static_cast<int64_t>(c.num_layers) * 12 * D +
              static_cast<int64_t>(c.num_single_layers) * 3 * D + 2 * D;
-  h->modW = ar.take(h->n_mod * D);
-  h->modB = ar.take(h->n_mod);
+  RF_TRY(h->mem.alloc(&h->modW, static_cast<size_t>(h->n_mod) * D));
+  RF_TRY(h->mem.alloc(&h->modB, h->n_mod));
 
   h->dbl.resize(c.num_layers);
   for (int i = 0; i < c.num_layers; ++i) {
@@ -277,10 +245,10 @@ int build_storage(rf_dit* h) {
     const int64_t mo = static_cast<int64_t>(i) * 12 * D;
     reg_lin(h, p + "norm1.linear", h->modW + mo * D, h->modB + mo, 6 * D, D);
     reg_lin(h, p + "norm1_context.linear", h->modW + (mo + 6 * D) * D, h->modB + mo + 6 * D, 6 * D, D);
-    new_pack(h, ar, b.l_norm1, {p + "norm1.linear"}, 6 * D, D, nullptr, false);
-    new_pack(h, ar, b.l_norm1c, {p + "norm1_context.linear"}, 6 * D, D, nullptr, true);
-    b.qkv = new_lin(h, ar, "", 3 * D, D);
-    b.add_qkv = new_lin(h, ar, "", 3 * D, D);
+    RF_TRY(new_pack(h, b.l_norm1, {p + "norm1.linear"}, 6 * D, D, nullptr, false));
+    RF_TRY(new_pack(h, b.l_norm1c, {p + "norm1_context.linear"}, 6 * D, D, nullptr, true));
+    RF_TRY(new_lin(h, b.qkv, "", 3 * D, D));
+    RF_TRY(new_lin(h, b.add_qkv, "", 3 * D, D));
     const char* nm[3] = {"to_q", "to_k", "to_v"};
     const char* an[3] = {"add_q_proj", "add_k_proj", "add_v_proj"};
     for (int j = 0; j < 3; ++j) {
@@ -288,25 +256,25 @@ int build_storage(rf_dit* h) {
       reg_lin(h, p + "attn." + an[j], b.add_qkv.w + static_cast<int64_t>(j) * D * D,
               b.add_qkv.b + j * D, D, D);
     }
-    new_pack(h, ar, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false);
-    new_pack(h, ar, b.l_add_qkv, {p + "attn.add_q_proj", p + "attn.add_k_proj", p + "attn.add_v_proj"}, D, D,
-             b.add_qkv.w, true);
-    b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
-    b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
-    b.norm_added_q = ar.take(128); reg(h, p + "attn.norm_added_q.weight", b.norm_added_q, 128);
-    b.norm_added_k = ar.take(128); reg(h, p + "attn.norm_added_k.weight", b.norm_added_k, 128);
-    b.to_out = new_lin(h, ar, p + "attn.to_out.0", D, D);
-    new_pack(h, ar, b.l_out, {p + "attn.to_out.0"}, D, D, b.to_out.w, false);
-    b.to_add_out = new_lin(h, ar, p + "attn.to_add_out", D, D);
-    new_pack(h, ar, b.l_add_out, {p + "attn.to_add_out"}, D, D, b.to_add_out.w, true);
-    b.ff1 = new_lin(h, ar, p + "ff.net.0.proj", 4 * D, D);
-    new_pack(h, ar, b.l_ff1, {p + "ff.net.0.proj"}, 4 * D, D, b.ff1.w, true);
-    b.ff2 = new_lin(h, ar, p + "ff.net.2", D, 4 * D);
-    new_pack(h, ar, b.l_ff2, {p + "ff.net.2"}, D, 4 * D, b.ff2.w, false);
-    b.ffc1 = new_lin(h, ar, p + "ff_context.net.0.proj", 4 * D, D);
-    b.ffc2 = new_lin(h, ar, p + "ff_context.net.2", D, 4 * D);
-    new_pack(h, ar, b.l_ffc1, {p + "ff_context.net.0.proj"}, 4 * D, D, b.ffc1.w, true);
-    new_pack(h, ar, b.l_ffc2, {p + "ff_context.net.2"}, D, 4 * D, b.ffc2.w, true);
+    RF_TRY(new_pack(h, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false));
+    RF_TRY(new_pack(h, b.l_add_qkv, {p + "attn.add_q_proj", p + "attn.add_k_proj", p + "attn.add_v_proj"}, D, D,
+                    b.add_qkv.w, true));
+    RF_TRY(new_vec(h, &b.norm_q, p + "attn.norm_q.weight", 128));
+    RF_TRY(new_vec(h, &b.norm_k, p + "attn.norm_k.weight", 128));
+    RF_TRY(new_vec(h, &b.norm_added_q, p + "attn.norm_added_q.weight", 128));
+    RF_TRY(new_vec(h, &b.norm_added_k, p + "attn.norm_added_k.weight", 128));
+    RF_TRY(new_lin(h, b.to_out, p + "attn.to_out.0", D, D));
+    RF_TRY(new_pack(h, b.l_out, {p + "attn.to_out.0"}, D, D, b.to_out.w, false));
+    RF_TRY(new_lin(h, b.to_add_out, p + "attn.to_add_out", D, D));
+    RF_TRY(new_pack(h, b.l_add_out, {p + "attn.to_add_out"}, D, D, b.to_add_out.w, true));
+    RF_TRY(new_lin(h, b.ff1, p + "ff.net.0.proj", 4 * D, D));
+    RF_TRY(new_pack(h, b.l_ff1, {p + "ff.net.0.proj"}, 4 * D, D, b.ff1.w, true));
+    RF_TRY(new_lin(h, b.ff2, p + "ff.net.2", D, 4 * D));
+    RF_TRY(new_pack(h, b.l_ff2, {p + "ff.net.2"}, D, 4 * D, b.ff2.w, false));
+    RF_TRY(new_lin(h, b.ffc1, p + "ff_context.net.0.proj", 4 * D, D));
+    RF_TRY(new_lin(h, b.ffc2, p + "ff_context.net.2", D, 4 * D));
+    RF_TRY(new_pack(h, b.l_ffc1, {p + "ff_context.net.0.proj"}, 4 * D, D, b.ffc1.w, true));
+    RF_TRY(new_pack(h, b.l_ffc2, {p + "ff_context.net.2"}, D, 4 * D, b.ffc2.w, true));
   }
   h->sgl.resize(c.num_single_layers);
   const int64_t so = static_cast<int64_t>(c.num_layers) * 12 * D;
@@ -315,29 +283,28 @@ int build_storage(rf_dit* h) {
     const std::string p = "single_transformer_blocks." + std::to_string(i) + ".";
     const int64_t mo = so + static_cast<int64_t>(i) * 3 * D;
     reg_lin(h, p + "norm.linear", h->modW + mo * D, h->modB + mo, 3 * D, D);
-    new_pack(h, ar, b.l_norm, {p + "norm.linear"}, 3 * D, D, nullptr, false);
-    b.qkv = new_lin(h, ar, "", 3 * D, D);
+    RF_TRY(new_pack(h, b.l_norm, {p + "norm.linear"}, 3 * D, D, nullptr, false));
+    RF_TRY(new_lin(h, b.qkv, "", 3 * D, D));
     const char* nm[3] = {"to_q", "to_k", "to_v"};
     for (int j = 0; j < 3; ++j)
       reg_lin(h, p + "attn." + nm[j], b.qkv.w + static_cast<int64_t>(j) * D * D, b.qkv.b + j * D, D, D);
-    b.mlp = new_lin(h, ar, p + "proj_mlp", 4 * D, D);
+    RF_TRY(new_lin(h, b.mlp, p + "proj_mlp", 4 * D, D));
     if (c.lora_rank > 0) {
       // A factors of to_q | to_k | to_v | proj_mlp stacked: all four read the same normalised tokens, so
       // ONE down-projection launch (NT = 4 lora_pad) serves the q|k|v and the MLP-in GEMMs of the block
-      b.l_qkv.A = ar.take(static_cast<int64_t>(4 * lpad) * D);
-      b.l_mlp.A = b.l_qkv.A ? b.l_qkv.A + static_cast<int64_t>(3 * lpad) * D : nullptr;
+      RF_TRY(h->mem.alloc(&b.l_qkv.A, static_cast<size_t>(4 * lpad) * D));
+      b.l_mlp.A = b.l_qkv.A + static_cast<int64_t>(3 * lpad) * D;
     }
-    new_pack(h, ar, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false);
-    new_pack(h, ar, b.l_mlp, {p + "proj_mlp"}, 4 * D, D, b.mlp.w, false);
-    b.norm_q = ar.take(128); reg(h, p + "attn.norm_q.weight", b.norm_q, 128);
-    b.norm_k = ar.take(128); reg(h, p + "attn.norm_k.weight", b.norm_k, 128);
-    b.out = new_lin(h, ar, p + "proj_out", D, 5 * D);
-    new_pack(h, ar, b.l_out, {p + "proj_out"}, D, 5 * D, b.out.w, false);
+    RF_TRY(new_pack(h, b.l_qkv, {p + "attn.to_q", p + "attn.to_k", p + "attn.to_v"}, D, D, b.qkv.w, false));
+    RF_TRY(new_pack(h, b.l_mlp, {p + "proj_mlp"}, 4 * D, D, b.mlp.w, false));
+    RF_TRY(new_vec(h, &b.norm_q, p + "attn.norm_q.weight", 128));
+    RF_TRY(new_vec(h, &b.norm_k, p + "attn.norm_k.weight", 128));
+    RF_TRY(new_lin(h, b.out, p + "proj_out", D, 5 * D));
+    RF_TRY(new_pack(h, b.l_out, {p + "proj_out"}, D, 5 * D, b.out.w, false));
   }
   const int64_t oo = so + static_cast<int64_t>(c.num_single_layers) * 3 * D;
   reg_lin(h, "norm_out.linear", h->modW + oo * D, h->modB + oo, 2 * D, D);
-  new_pack(h, ar, h->l_norm_out, {"norm_out.linear"}, 2 * D, D, nullptr, true);
-  return ar.fail;
+  return new_pack(h, h->l_norm_out, {"norm_out.linear"}, 2 * D, D, nullptr, true);
 }
 
 // modulation vector offsets inside MOD / MODC
@@ -495,11 +462,7 @@ int merge_all(rf_dit* h, cudaStream_t s) {
   for (LoraPack* p : h->proj_packs) {
     if (!pack_set(*p)) continue;
     const size_t elems = static_cast<size_t>(p->t[0].out) * p->t[0].in;
-    if (p->Wm == nullptr) {
-      void* q = nullptr;
-      if (dev_alloc(h, &q, p->n * elems * 2)) return -2;
-      p->Wm = static_cast<bf16*>(q);
-    }
+    if (p->Wm == nullptr) RF_TRY(h->mem.alloc(&p->Wm, p->n * elems));
     for (int k = 0; k < p->n; ++k) {
       const LoraT& t = p->t[k];
       const size_t off = k * elems;
@@ -766,11 +729,8 @@ int lora_rows_needed(const rf_dit* h, int flags, int N, int n_cond) {
 // LT [rows, 4 lora_pad] and LL [rows, 4D]
 int alloc_lora_ws(rf_dit* h, int rows) {
   const size_t r = static_cast<size_t>(rows);
-  void* p = nullptr;
-  RF_TRY(dev_alloc(h, &p, r * 4 * h->lora_pad * 2, true));
-  h->LT = static_cast<bf16*>(p);
-  RF_TRY(dev_alloc(h, &p, r * 4 * h->D * 2, true));
-  h->LL = static_cast<bf16*>(p);
+  RF_TRY(h->geo_mem.alloc(&h->LT, r * 4 * h->lora_pad));
+  RF_TRY(h->geo_mem.alloc(&h->LL, r * 4 * h->D));
   h->lora_rows = rows;
   return 0;
 }
@@ -787,8 +747,7 @@ void drop_graph(rf_dit* h) {
 }
 void free_geometry(rf_dit* h) {
   drop_graph(h);
-  for (void* p : h->geo_allocs) cudaFree(p);
-  h->geo_allocs.clear();
+  h->geo_mem.release_all();
   h->prepared = false;
   h->lora_rows = 0;
   h->s_cap_steps = 0;
@@ -909,11 +868,7 @@ int rf_dit_create(const rf_dit_config* cfg, rf_dit** out) {
     rf::set_error("rf_dit_create: lora_rank must be 0..128, got " + std::to_string(cfg->lora_rank));
     return -1;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    rf::set_error("rf_dit_create: no CUDA device (this library has no CPU fallback)");
-    return -3;
-  }
+  RF_TRY(rf::require_device("rf_dit_create"));
   if (cfg->num_heads <= 0 || cfg->in_channels % 64 != 0 || cfg->joint_attention_dim % 64 != 0 ||
       cfg->pooled_projection_dim % 8 != 0) {
     rf::set_error("rf_dit_create: unsupported config");
@@ -947,10 +902,8 @@ int rf_dit_create(const rf_dit_config* cfg, rf_dit** out) {
 void rf_dit_destroy(rf_dit* h) {
   if (!h) return;
   free_geometry(h);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
-  if (h->ev_in) cudaEventDestroy(h->ev_in);
-  if (h->ev_out) cudaEventDestroy(h->ev_out);
-  for (void* p : h->allocs) cudaFree(p);
+  h->side.destroy();
+  h->mem.release_all();
   delete h;
 }
 
@@ -959,19 +912,7 @@ int rf_dit_load_weight(rf_dit* h, const char* key, const void* src, int64_t nume
     rf::set_error("rf_dit_load_weight: null argument");
     return -1;
   }
-  auto it = h->slots.find(key);
-  if (it == h->slots.end()) {
-    rf::set_error(std::string("rf_dit_load_weight: unknown key ") + key);
-    return -4;
-  }
-  if (it->second.numel != numel) {
-    rf::set_error(std::string("rf_dit_load_weight: size mismatch for ") + key + ": got " +
-                  std::to_string(numel) + ", want " + std::to_string(it->second.numel));
-    return -4;
-  }
-  RF_CHECK_CUDA(cudaMemcpy(it->second.dst, src, static_cast<size_t>(numel) * 2,
-                           cudaMemcpyDeviceToDevice));
-  it->second.loaded = true;
+  RF_TRY(h->weights.load("rf_dit_load_weight", key, src, numel));
   h->lora_merged = false;  // merged W + BA copies (fuse_lora mode) are stale now
   return 0;
 }
@@ -1059,19 +1000,7 @@ int rf_dit_set_lora_scale(rf_dit* h, double scale) {
   return 0;
 }
 
-int rf_dit_missing_weights(rf_dit* h) {
-  if (!h) return -1;
-  int missing = 0;
-  std::string names;
-  for (auto& kv : h->slots) {
-    if (!kv.second.loaded) {
-      if (missing < 8) names += kv.first + " ";
-      ++missing;
-    }
-  }
-  if (missing) rf::set_error("missing weights: " + names + (missing > 8 ? "..." : ""));
-  return missing;
-}
+int rf_dit_missing_weights(rf_dit* h) { return h ? h->weights.missing("", "missing weights") : -1; }
 
 int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const void* txt_ids,
                    const void* img_ids, const void* cond_ids, int flags, float condition_scale,
@@ -1117,37 +1046,33 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     h->prepared = false;
     h->batch = batch; h->n_txt = n_txt; h->n_img = n_img; h->n_cond = n_cond;
     h->N = N; h->n_main = n_main;
-    void* p;
-    auto A = [&](size_t bytes) -> void* {
-      void* q = nullptr;
-      if (dev_alloc(h, &q, bytes, true)) return nullptr;
-      return q;
-    };
-    if (!(p = A(static_cast<size_t>(n_main) * 64 * 4))) return -2; h->rope_cos = static_cast<float*>(p);
-    if (!(p = A(static_cast<size_t>(n_main) * 64 * 4))) return -2; h->rope_sin = static_cast<float*>(p);
-    if (!(p = A(static_cast<size_t>(std::max(n_cond, 1)) * 64 * 4))) return -2; h->crope_cos = static_cast<float*>(p);
-    if (!(p = A(static_cast<size_t>(std::max(n_cond, 1)) * 64 * 4))) return -2; h->crope_sin = static_cast<float*>(p);
-    if (!(p = A(static_cast<size_t>(N) * D * 2))) return -2; h->X = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(N) * D * 2))) return -2; h->XN = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(N) * 3 * D * 2))) return -2; h->QKV = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(N) * 5 * D * 2))) return -2; h->ACT = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MOD = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(h->n_mod) * 2))) return -2; h->MODC = static_cast<bf16*>(p);
+    rf::DeviceAllocs& g = h->geo_mem;
+    const size_t nc = std::max(n_cond, 1);
+    RF_TRY(g.alloc(&h->rope_cos, static_cast<size_t>(n_main) * 64));
+    RF_TRY(g.alloc(&h->rope_sin, static_cast<size_t>(n_main) * 64));
+    RF_TRY(g.alloc(&h->crope_cos, nc * 64));
+    RF_TRY(g.alloc(&h->crope_sin, nc * 64));
+    RF_TRY(g.alloc(&h->X, static_cast<size_t>(N) * D));
+    RF_TRY(g.alloc(&h->XN, static_cast<size_t>(N) * D));
+    RF_TRY(g.alloc(&h->QKV, static_cast<size_t>(N) * 3 * D));
+    RF_TRY(g.alloc(&h->ACT, static_cast<size_t>(N) * 5 * D));
+    RF_TRY(g.alloc(&h->MOD, h->n_mod));
+    RF_TRY(g.alloc(&h->MODC, h->n_mod));
     RF_TRY(alloc_lora_ws(h, lora_rows));
-    if (!(p = A(static_cast<size_t>(temb_ws_elems(h, 1)) * 2))) return -2; h->emb_ws = static_cast<bf16*>(p);
+    RF_TRY(g.alloc(&h->emb_ws, temb_ws_elems(h, 1)));
     const int C = h->cfg.in_channels;
-    if (!(p = A(static_cast<size_t>(batch) * n_img * C * 2))) return -2; h->s_lat = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(batch) * n_img * C * 2))) return -2; h->s_v = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(batch) * n_txt * h->cfg.joint_attention_dim * 2))) return -2; h->s_txt = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(batch) * h->cfg.pooled_projection_dim * 2))) return -2; h->s_pooled = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(batch) * std::max(n_cond, 1) * C * 2))) return -2; h->s_cond = static_cast<bf16*>(p);
-    if (!(p = A(static_cast<size_t>(batch) * 2 + 16))) return -2; h->s_guid = static_cast<bf16*>(p);
-    if (!(p = A(16))) return -2; h->s_zero_one = static_cast<bf16*>(p);
-    if (!(p = A(16))) return -2; h->s_step = static_cast<int*>(p);
+    RF_TRY(g.alloc(&h->s_lat, static_cast<size_t>(batch) * n_img * C));
+    RF_TRY(g.alloc(&h->s_v, static_cast<size_t>(batch) * n_img * C));
+    RF_TRY(g.alloc(&h->s_txt, static_cast<size_t>(batch) * n_txt * h->cfg.joint_attention_dim));
+    RF_TRY(g.alloc(&h->s_pooled, static_cast<size_t>(batch) * h->cfg.pooled_projection_dim));
+    RF_TRY(g.alloc(&h->s_cond, batch * nc * C));
+    RF_TRY(g.alloc(&h->s_guid, static_cast<size_t>(batch) + 8));
+    RF_TRY(g.alloc(&h->s_zero_one, 8));
+    RF_TRY(g.alloc(&h->s_step, 4));
     if (n_cond > 0) {  // image guidance needs a condition stream
-      if (!(p = A(static_cast<size_t>(n_cond) * C * 2))) return -2; h->s_ucond = static_cast<bf16*>(p);
-      if (!(p = A(static_cast<size_t>(n_img) * C * 2))) return -2; h->s_vu = static_cast<bf16*>(p);
-      if (!(p = A(16))) return -2; h->s_igs = static_cast<float*>(p);
+      RF_TRY(g.alloc(&h->s_ucond, static_cast<size_t>(n_cond) * C));
+      RF_TRY(g.alloc(&h->s_vu, static_cast<size_t>(n_img) * C));
+      RF_TRY(g.alloc(&h->s_igs, 4));
     }
     h->s_cap_steps = 0;
     h->s_tsteps = nullptr;
@@ -1196,11 +1121,8 @@ static int check_ready(rf_dit* h, const char* who, cudaStream_t s) {
   const int rows = lora_rows_needed(h, h->flags, h->N, h->n_cond);
   if (rows > h->lora_rows) {
     drop_graph(h);
-    for (bf16* old : {h->LT, h->LL}) {
-      auto it = std::find(h->geo_allocs.begin(), h->geo_allocs.end(), static_cast<void*>(old));
-      if (it != h->geo_allocs.end()) h->geo_allocs.erase(it);
-      cudaFree(old);
-    }
+    h->geo_mem.release(h->LT);
+    h->geo_mem.release(h->LL);
     RF_TRY(alloc_lora_ws(h, rows));
   }
   // fuse_lora mode: weights or adapters changed since the last merge -> re-merge before use
@@ -1248,40 +1170,20 @@ int rf_dit_forward(rf_dit* h, const void* latents, const void* txt, const void* 
 static int capture_step(rf_dit* h, bool guided, StepGraph* g, cudaStream_t s) {
   const int C = h->cfg.in_channels;
   g->call_scale = h->call_scale;
-  cudaGraph_t graph = nullptr;
-  const int64_t launches_before = rf::launch_count();
-  RF_CHECK_CUDA(cudaStreamSynchronize(s));
-  RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-  int erc = enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_guid,
-                            h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s, h->s_mod_all);
-  if (guided) {
-    if (!erc) erc = enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_zero_one + 1,
-                                    h->s_ucond, h->s_vu, s, h->s_mod_all_u);
-    if (!erc) erc = rf::image_guidance_step_launch(h->s_lat, h->s_v, h->s_vu, h->s_igs, h->s_sigmas, h->s_step,
-                                                   h->n_img * C, s);
-  } else if (!erc) {
-    erc = rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s);
-  }
-  if (!erc) erc = rf::advance_step_launch(h->s_step, s);
-  cudaError_t ce = cudaStreamEndCapture(s, &graph);
-  if (erc || ce != cudaSuccess) {
-    if (graph) cudaGraphDestroy(graph);
-    if (!erc) {
-      rf::set_error(std::string("graph capture failed: ") + cudaGetErrorString(ce));
-      erc = -2;
+  auto step = [&]() {
+    RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_guid,
+                           h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s, h->s_mod_all));
+    if (guided) {
+      RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_zero_one + 1,
+                             h->s_ucond, h->s_vu, s, h->s_mod_all_u));
+      RF_TRY(rf::image_guidance_step_launch(h->s_lat, h->s_v, h->s_vu, h->s_igs, h->s_sigmas, h->s_step,
+                                            h->n_img * C, s));
+    } else {
+      RF_TRY(rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s));
     }
-    return erc;
-  }
-  g->kernels = rf::launch_count() - launches_before;
-  rf::count_launch(static_cast<int>(-g->kernels));  // captured, not executed
-  ce = cudaGraphInstantiate(&g->exec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (ce != cudaSuccess) {
-    g->exec = nullptr;
-    rf::set_error(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ce));
-    return -2;
-  }
-  return 0;
+    return rf::advance_step_launch(h->s_step, s);
+  };
+  return rf::capture_graph(s, "rf_dit", step, &g->exec, &g->kernels);
 }
 
 // rf_dit_denoise, and with uncond_latents != nullptr rf_dit_denoise_image_guidance (arguments checked by the caller)
@@ -1290,36 +1192,21 @@ static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const v
                         float guidance_scale, const void* cond_latents, const bf16* uncond_latents,
                         float image_guidance_scale, void* stream) {
   const bool guided = uncond_latents != nullptr;
-  // The loop runs on a handle-owned stream (graph capture is not permitted on the legacy default
-  // stream callers often pass); it is ordered after / before the caller's stream with events, so
-  // the call still only enqueues work.
+  // The loop runs on the handle's side stream, so the step can be captured whatever stream the caller passes
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  if (!h->own_stream) {
-    RF_CHECK_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-  }
-  cudaStream_t s = h->own_stream;
-  RF_CHECK_CUDA(cudaEventRecord(h->ev_in, caller));
-  RF_CHECK_CUDA(cudaStreamWaitEvent(s, h->ev_in, 0));
+  cudaStream_t s = nullptr;
+  RF_TRY(h->side.enter(caller, &s));
   const int C = h->cfg.in_channels;
   if (n_steps > h->s_cap_steps) {
-    void* p = nullptr;
-    if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * 2, true)) return -2;
-    h->s_tsteps = static_cast<bf16*>(p);
-    if (dev_alloc(h, &p, static_cast<size_t>(n_steps + 1) * 4, true)) return -2;
-    h->s_sigmas = static_cast<float*>(p);
-    if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
-    h->s_mod_all = static_cast<bf16*>(p);
-    if (dev_alloc(h, &p, static_cast<size_t>(temb_ws_elems(h, n_steps)) * 2, true)) return -2;
-    h->s_temb_ws = static_cast<bf16*>(p);
+    RF_TRY(h->geo_mem.alloc(&h->s_tsteps, n_steps));
+    RF_TRY(h->geo_mem.alloc(&h->s_sigmas, n_steps + 1));
+    RF_TRY(h->geo_mem.alloc(&h->s_mod_all, static_cast<size_t>(n_steps) * h->n_mod));
+    RF_TRY(h->geo_mem.alloc(&h->s_temb_ws, temb_ws_elems(h, n_steps)));
     h->s_cap_steps = n_steps;
     drop_graph(h);  // graph referenced the old arrays
   }
   if (guided && n_steps > h->s_cap_steps_u) {
-    void* p = nullptr;
-    if (dev_alloc(h, &p, static_cast<size_t>(n_steps) * h->n_mod * 2, true)) return -2;
-    h->s_mod_all_u = static_cast<bf16*>(p);
+    RF_TRY(h->geo_mem.alloc(&h->s_mod_all_u, static_cast<size_t>(n_steps) * h->n_mod));
     h->s_cap_steps_u = n_steps;
     drop_graph(h);
   }
@@ -1374,9 +1261,7 @@ static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const v
     RF_CHECK_CUDA(cudaMemcpyAsync(lat_b, h->s_lat, static_cast<size_t>(h->n_img) * C * 2,
                                   cudaMemcpyDeviceToDevice, s));
   }
-  RF_CHECK_CUDA(cudaEventRecord(h->ev_out, s));
-  RF_CHECK_CUDA(cudaStreamWaitEvent(caller, h->ev_out, 0));
-  return 0;
+  return h->side.leave(caller);
 }
 
 int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,

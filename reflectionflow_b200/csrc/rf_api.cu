@@ -1,5 +1,7 @@
 #include <cstdlib>
-// rf_api.cu — operator-level C ABI (include/rf_b200.h) over the kernel launchers.
+// rf_api.cu — operator-level C ABI (include/rf_b200.h) over the kernel launchers, and the host plumbing the
+// handles share (rf_internal.h).
+#include <algorithm>
 #include <atomic>
 #include <cstring>
 #include <map>
@@ -21,6 +23,115 @@ const char* get_error() { return g_err.c_str(); }
 static std::atomic<int64_t> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
+
+int require_device(const char* who) {
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    set_error(std::string(who) + ": no CUDA device (this library has no CPU fallback)");
+    return -3;
+  }
+  return 0;
+}
+
+void DeviceAllocs::release(void* p) {
+  auto it = std::find(blocks_.begin(), blocks_.end(), p);
+  if (it == blocks_.end()) return;
+  blocks_.erase(it);
+  cudaFree(p);
+}
+void DeviceAllocs::release_all() {
+  for (void* p : blocks_) cudaFree(p);
+  blocks_.clear();
+}
+
+void WeightTable::add(const std::string& key, bf16* dst, int64_t numel, ConvRepack conv) {
+  entries_[key] = Entry{dst, numel, conv, false};
+}
+int WeightTable::load(const char* who, const char* key, const void* src, int64_t numel) {
+  auto it = entries_.find(key);
+  if (it == entries_.end()) {
+    set_error(std::string(who) + ": unknown key " + key);
+    return -4;
+  }
+  Entry& e = it->second;
+  if (e.numel != numel) {
+    set_error(std::string(who) + ": size mismatch for " + key + ": got " + std::to_string(numel) + ", want " +
+              std::to_string(e.numel));
+    return -4;
+  }
+  const ConvRepack& c = e.conv;
+  if (c.taps > 0)
+    RF_TRY(conv_repack_launch(static_cast<const bf16*>(src), e.dst, c.cout, c.cin, c.taps, c.cout_pad, c.cin_pad,
+                              nullptr));
+  else
+    RF_CHECK_CUDA(cudaMemcpy(e.dst, src, static_cast<size_t>(numel) * 2, cudaMemcpyDeviceToDevice));
+  e.loaded = true;
+  return 0;
+}
+int WeightTable::missing(const char* prefix, const char* what) const {
+  int n = 0;
+  std::string names;
+  const size_t pl = strlen(prefix);
+  for (auto& kv : entries_)
+    if (!kv.second.loaded && kv.first.compare(0, pl, prefix) == 0) {
+      if (n < 8) names += kv.first + " ";
+      ++n;
+    }
+  if (n) set_error(std::string(what) + ": " + names + (n > 8 ? "..." : ""));
+  return n;
+}
+
+int SideStream::enter(cudaStream_t caller, cudaStream_t* s) {
+  if (!stream_) {
+    RF_CHECK_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+    RF_CHECK_CUDA(cudaEventCreateWithFlags(&ev_in_, cudaEventDisableTiming));
+    RF_CHECK_CUDA(cudaEventCreateWithFlags(&ev_out_, cudaEventDisableTiming));
+  }
+  RF_CHECK_CUDA(cudaEventRecord(ev_in_, caller));
+  RF_CHECK_CUDA(cudaStreamWaitEvent(stream_, ev_in_, 0));
+  *s = stream_;
+  return 0;
+}
+int SideStream::leave(cudaStream_t caller) {
+  RF_CHECK_CUDA(cudaEventRecord(ev_out_, stream_));
+  RF_CHECK_CUDA(cudaStreamWaitEvent(caller, ev_out_, 0));
+  return 0;
+}
+void SideStream::destroy() {
+  if (stream_) cudaStreamDestroy(stream_);
+  if (ev_in_) cudaEventDestroy(ev_in_);
+  if (ev_out_) cudaEventDestroy(ev_out_);
+  stream_ = nullptr;
+  ev_in_ = ev_out_ = nullptr;
+}
+
+int capture_graph(cudaStream_t s, const char* who, const std::function<int()>& body, cudaGraphExec_t* exec,
+                  int64_t* launches) {
+  RF_CHECK_CUDA(cudaStreamSynchronize(s));
+  const int64_t before = launch_count();
+  RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+  int rc = body();
+  cudaGraph_t graph = nullptr;
+  cudaError_t ce = cudaStreamEndCapture(s, &graph);
+  *launches = launch_count() - before;
+  count_launch(static_cast<int>(-*launches));  // captured, not executed
+  if (rc || ce != cudaSuccess) {
+    if (graph) cudaGraphDestroy(graph);
+    if (!rc) {
+      set_error(std::string(who) + ": graph capture failed: " + cudaGetErrorString(ce));
+      rc = -2;
+    }
+    return rc;
+  }
+  ce = cudaGraphInstantiate(exec, graph, 0);
+  cudaGraphDestroy(graph);
+  if (ce != cudaSuccess) {
+    *exec = nullptr;
+    set_error(std::string(who) + ": cudaGraphInstantiate: " + cudaGetErrorString(ce));
+    return -2;
+  }
+  return 0;
+}
 
 struct ProfRec {
   const char* name;

@@ -1,5 +1,5 @@
 // rf_internal.h — host-side declarations shared by the kernel translation units and the
-// DiT orchestrator.  Nothing here is part of the public C ABI (see include/rf_b200.h).
+// DiT, VAE and text-encoder handles.  Nothing here is part of the public C ABI (see include/rf_b200.h).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -7,7 +7,10 @@
 #include <stdint.h>
 
 #include <cstring>
+#include <functional>
 #include <string>
+#include <unordered_map>
+#include <vector>
 
 namespace rf {
 
@@ -28,6 +31,79 @@ int64_t launch_count();
       return -2;                                                                         \
     }                                                                                    \
   } while (0)
+
+// return the status of an rf call that failed (nonzero), its error already set
+#define RF_TRY(expr)            \
+  do {                          \
+    int _rc = (expr);           \
+    if (_rc != 0) return _rc;   \
+  } while (0)
+
+// -3 with "<who>: no CUDA device" when there is none (this library has no CPU fallback)
+int require_device(const char* who);
+
+// The device memory a handle owns.  Every block stays allocated until release(p) or release_all().
+class DeviceAllocs {
+ public:
+  // *p = `count` new elements of T (an empty request still takes 16 bytes); -2 and the CUDA error on failure
+  template <typename T>
+  int alloc(T** p, size_t count) {
+    void* q = nullptr;
+    RF_CHECK_CUDA(cudaMalloc(&q, count ? count * sizeof(T) : 16));
+    blocks_.push_back(q);
+    *p = static_cast<T*>(q);
+    return 0;
+  }
+  void release(void* p);  // frees p if this list owns it
+  void release_all();
+
+ private:
+  std::vector<void*> blocks_;
+};
+
+// How a VAE convolution weight is stored (conv_repack_launch): torch [cout, cin, kh, kw] -> [cout_pad, taps * cin_pad]
+struct ConvRepack {
+  int cout = 0, cin = 0, taps = 0, cout_pad = 0, cin_pad = 0;
+};
+
+// The named weights of a handle: what rf_*_load_weight writes and rf_*_missing_weights counts.  An entry is a
+// device range of its own or a row slice of a stacked buffer; each key is marked loaded on its own.
+class WeightTable {
+ public:
+  // numel elements at dst; a `conv` with taps > 0 is repacked into its device layout on load instead of copied
+  void add(const std::string& key, bf16* dst, int64_t numel, ConvRepack conv = {});
+  // who: the entry point, for the error text.  -4 on an unknown key or a size mismatch.
+  int load(const char* who, const char* key, const void* src, int64_t numel);
+  // the number of keys under `prefix` not loaded yet; if any, the error "<what>: <the first few keys>"
+  int missing(const char* prefix, const char* what) const;
+
+ private:
+  struct Entry {
+    bf16* dst;
+    int64_t numel;
+    ConvRepack conv;
+    bool loaded;
+  };
+  std::unordered_map<std::string, Entry> entries_;
+};
+
+// A handle's private stream (graph capture is illegal on the legacy default stream callers often pass).  enter()
+// orders it after the caller's stream, leave() the caller after it, so a call still only enqueues work.
+class SideStream {
+ public:
+  int enter(cudaStream_t caller, cudaStream_t* s);  // creates the stream and its events on first use
+  int leave(cudaStream_t caller);
+  void destroy();
+
+ private:
+  cudaStream_t stream_ = nullptr;
+  cudaEvent_t ev_in_ = nullptr, ev_out_ = nullptr;
+};
+
+// Capture what `body` enqueues on s (a thread-local capture) into *exec.  The launches body counts are captured, not
+// executed: they are taken off rf_launch_count() and returned in *launches.  who: prefix of the error text.
+int capture_graph(cudaStream_t s, const char* who, const std::function<int()>& body, cudaGraphExec_t* exec,
+                  int64_t* launches);
 
 // Launch with programmatic stream serialization (PDL) unless RF_PDL=0: the kernel MUST call
 // pdl_wait() (rf_ptx.cuh) before its first global-memory access.

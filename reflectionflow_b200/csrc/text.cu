@@ -15,7 +15,6 @@
 #include <cmath>
 #include <cstring>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/rf_b200.h"
@@ -352,15 +351,14 @@ int text_gather_rows_launch(const bf16* x, const int* pos, bf16* out, int B, int
 using rf::bf16;
 
 namespace {
-struct TSlot { bf16* dst; int64_t numel; bool loaded; };
 struct T5Layer { bf16 *qkv, *o, *ln0, *wi0, *wi1, *wo, *ln1; };
 struct ClipLayer { bf16 *ln1w, *ln1b, *qkvw, *qkvb, *ow, *ob, *ln2w, *ln2b, *fc1w, *fc1b, *fc2w, *fc2b; };
 }  // namespace
 
 struct rf_text {
   rf_text_config cfg;
-  std::vector<void*> allocs;
-  std::unordered_map<std::string, TSlot> slots;
+  rf::DeviceAllocs mem;
+  rf::WeightTable weights;
   // T5
   bf16 *t5_shared = nullptr, *t5_final = nullptr;
   std::vector<T5Layer> t5;
@@ -375,25 +373,12 @@ struct rf_text {
 };
 
 namespace {
-#define RF_TRYT(expr)           \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != 0) return _rc;   \
-  } while (0)
-
-int talloc(rf_text* h, void** p, size_t bytes) {
-  RF_CHECK_CUDA(cudaMalloc(p, bytes ? bytes : 16));
-  h->allocs.push_back(*p);
+// a weight's own storage, registered under `key`
+int new_weight(rf_text* h, bf16** p, int64_t n, const std::string& key) {
+  RF_TRY(h->mem.alloc(p, n));
+  h->weights.add(key, *p, n);
   return 0;
 }
-bf16* take(rf_text* h, int64_t n, int& rc, const std::string& key = "") {
-  void* p = nullptr;
-  if (talloc(h, &p, static_cast<size_t>(n) * 2)) rc = -2;
-  if (!key.empty()) h->slots[key] = {static_cast<bf16*>(p), n, false};
-  return static_cast<bf16*>(p);
-}
-// a slice of a packed matrix registered under its own key
-void alias(rf_text* h, const std::string& key, bf16* p, int64_t n) { h->slots[key] = {p, n, false}; }
 
 int linear(int epi, const bf16* A, int lda, int M, const bf16* W, const bf16* bias, bf16* out, int ldo, int N,
            int K, const bf16* res, int ldr, const bf16* ones, cudaStream_t s) {
@@ -434,28 +419,73 @@ int ensure_ws(rf_text* h, int tokens) {
   const int D = c.t5_d_model > c.clip_d_model ? c.t5_d_model : c.clip_d_model;
   const int F = c.t5_d_ff > 4 * c.clip_d_model ? c.t5_d_ff : 4 * c.clip_d_model;
   const int QKV = 3 * (c.t5_heads * 64 > c.clip_d_model ? c.t5_heads * 64 : c.clip_d_model);
-  void* p;
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * D * 2)); h->x = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * D * 2)); h->xn = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * QKV * 2)); h->qkv = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * D * 2)); h->att = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * F * 2)); h->h0 = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * F * 2)); h->h1 = static_cast<bf16*>(p);
-  RF_TRYT(talloc(h, &p, static_cast<size_t>(tokens) * 4)); h->ids = static_cast<int*>(p);
+  RF_TRY(h->mem.alloc(&h->x, static_cast<size_t>(tokens) * D));
+  RF_TRY(h->mem.alloc(&h->xn, static_cast<size_t>(tokens) * D));
+  RF_TRY(h->mem.alloc(&h->qkv, static_cast<size_t>(tokens) * QKV));
+  RF_TRY(h->mem.alloc(&h->att, static_cast<size_t>(tokens) * D));
+  RF_TRY(h->mem.alloc(&h->h0, static_cast<size_t>(tokens) * F));
+  RF_TRY(h->mem.alloc(&h->h1, static_cast<size_t>(tokens) * F));
+  RF_TRY(h->mem.alloc(&h->ids, tokens));
   h->ws_tokens = tokens;
   return 0;
 }
-int missing(rf_text* h, const char* prefix) {
-  int n = 0;
-  std::string names;
-  const size_t pl = strlen(prefix);
-  for (auto& kv : h->slots)
-    if (kv.first.compare(0, pl, prefix) == 0 && !kv.second.loaded) {
-      if (n < 6) names += kv.first + " ";
-      ++n;
+
+// the weights of both encoders, each under its transformers key
+int build_weights(rf_text* h) {
+  const rf_text_config& c = h->cfg;
+  const int D = c.t5_d_model, F = c.t5_d_ff, I = c.t5_heads * 64;
+  RF_TRY(new_weight(h, &h->t5_shared, static_cast<int64_t>(c.t5_vocab) * D, "t5.shared.weight"));
+  h->t5.resize(c.t5_layers);
+  for (int i = 0; i < c.t5_layers; ++i) {
+    T5Layer& L = h->t5[i];
+    const std::string p = "t5.encoder.block." + std::to_string(i) + ".layer.";
+    const int64_t ID = static_cast<int64_t>(I) * D;
+    RF_TRY(h->mem.alloc(&L.qkv, 3 * ID));  // q | k | v stacked, each registered as its rows
+    h->weights.add(p + "0.SelfAttention.q.weight", L.qkv, ID);
+    h->weights.add(p + "0.SelfAttention.k.weight", L.qkv + ID, ID);
+    h->weights.add(p + "0.SelfAttention.v.weight", L.qkv + 2 * ID, ID);
+    RF_TRY(new_weight(h, &L.o, ID, p + "0.SelfAttention.o.weight"));
+    RF_TRY(new_weight(h, &L.ln0, D, p + "0.layer_norm.weight"));
+    RF_TRY(new_weight(h, &L.wi0, static_cast<int64_t>(F) * D, p + "1.DenseReluDense.wi_0.weight"));
+    RF_TRY(new_weight(h, &L.wi1, static_cast<int64_t>(F) * D, p + "1.DenseReluDense.wi_1.weight"));
+    RF_TRY(new_weight(h, &L.wo, static_cast<int64_t>(D) * F, p + "1.DenseReluDense.wo.weight"));
+    RF_TRY(new_weight(h, &L.ln1, D, p + "1.layer_norm.weight"));
+  }
+  RF_TRY(new_weight(h, &h->t5_final, D, "t5.encoder.final_layer_norm.weight"));
+  const int C = c.clip_d_model;
+  const int64_t CC = static_cast<int64_t>(C) * C;
+  RF_TRY(new_weight(h, &h->clip_tok, static_cast<int64_t>(c.clip_vocab) * C,
+                    "clip.text_model.embeddings.token_embedding.weight"));
+  RF_TRY(new_weight(h, &h->clip_pos, static_cast<int64_t>(c.clip_max_pos) * C,
+                    "clip.text_model.embeddings.position_embedding.weight"));
+  h->clip.resize(c.clip_layers);
+  for (int i = 0; i < c.clip_layers; ++i) {
+    ClipLayer& L = h->clip[i];
+    const std::string p = "clip.text_model.encoder.layers." + std::to_string(i) + ".";
+    RF_TRY(new_weight(h, &L.ln1w, C, p + "layer_norm1.weight"));
+    RF_TRY(new_weight(h, &L.ln1b, C, p + "layer_norm1.bias"));
+    RF_TRY(h->mem.alloc(&L.qkvw, 3 * CC));  // q | k | v stacked, each registered as its rows
+    RF_TRY(h->mem.alloc(&L.qkvb, 3 * C));
+    const char* nm[3] = {"q_proj", "k_proj", "v_proj"};
+    for (int j = 0; j < 3; ++j) {
+      h->weights.add(p + "self_attn." + nm[j] + ".weight", L.qkvw + j * CC, CC);
+      h->weights.add(p + "self_attn." + nm[j] + ".bias", L.qkvb + j * C, C);
     }
-  if (n) rf::set_error("missing text-encoder weights: " + names);
-  return n;
+    RF_TRY(new_weight(h, &L.ow, CC, p + "self_attn.out_proj.weight"));
+    RF_TRY(new_weight(h, &L.ob, C, p + "self_attn.out_proj.bias"));
+    RF_TRY(new_weight(h, &L.ln2w, C, p + "layer_norm2.weight"));
+    RF_TRY(new_weight(h, &L.ln2b, C, p + "layer_norm2.bias"));
+    RF_TRY(new_weight(h, &L.fc1w, 4 * CC, p + "mlp.fc1.weight"));
+    RF_TRY(new_weight(h, &L.fc1b, 4 * C, p + "mlp.fc1.bias"));
+    RF_TRY(new_weight(h, &L.fc2w, 4 * CC, p + "mlp.fc2.weight"));
+    RF_TRY(new_weight(h, &L.fc2b, C, p + "mlp.fc2.bias"));
+  }
+  RF_TRY(new_weight(h, &h->clip_fw, C, "clip.text_model.final_layer_norm.weight"));
+  RF_TRY(new_weight(h, &h->clip_fb, C, "clip.text_model.final_layer_norm.bias"));
+  RF_TRY(h->mem.alloc(&h->ones, 4096));
+  const std::vector<uint16_t> one(4096, 0x3F80);
+  RF_CHECK_CUDA(cudaMemcpy(h->ones, one.data(), 8192, cudaMemcpyHostToDevice));
+  return 0;
 }
 }  // namespace
 
@@ -463,8 +493,8 @@ namespace rf {
 // T5DenseGatedActDense up to wo: h0 = bf16(x wi_0^T), h1 = bf16(x wi_1^T), h0 = bf16(gelu_new(h0) * h1)
 int t5_gated_gelu(const bf16* x, int T, int D, const bf16* wi0, const bf16* wi1, int F, bf16* h0, bf16* h1,
                   cudaStream_t s) {
-  RF_TRYT(linear(EPI_BIAS, x, D, T, wi0, nullptr, h0, F, F, D, nullptr, 0, nullptr, s));
-  RF_TRYT(linear(EPI_BIAS, x, D, T, wi1, nullptr, h1, F, F, D, nullptr, 0, nullptr, s));
+  RF_TRY(linear(EPI_BIAS, x, D, T, wi0, nullptr, h0, F, F, D, nullptr, 0, nullptr, s));
+  RF_TRY(linear(EPI_BIAS, x, D, T, wi1, nullptr, h1, F, F, D, nullptr, 0, nullptr, s));
   return text_ewise_launch(h0, h1, h0, static_cast<int64_t>(T) * F, 0, s);
 }
 }  // namespace rf
@@ -476,11 +506,7 @@ int rf_text_create(const rf_text_config* cfg, rf_text** out) {
     rf::set_error("rf_text_create: null argument");
     return -1;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    rf::set_error("rf_text_create: no CUDA device (this library has no CPU fallback)");
-    return -3;
-  }
+  RF_TRY(rf::require_device("rf_text_create"));
   if (cfg->t5_d_model % 256 || cfg->t5_d_ff % 256 || cfg->clip_d_model % 256 || cfg->t5_d_model > 4096 ||
       cfg->clip_heads * 64 != cfg->clip_d_model) {
     rf::set_error("rf_text_create: unsupported config (widths must be multiples of 256, head_dim 64)");
@@ -488,57 +514,7 @@ int rf_text_create(const rf_text_config* cfg, rf_text** out) {
   }
   rf_text* h = new rf_text();
   h->cfg = *cfg;
-  int rc = 0;
-  const int D = cfg->t5_d_model, F = cfg->t5_d_ff, I = cfg->t5_heads * 64;
-  h->t5_shared = take(h, static_cast<int64_t>(cfg->t5_vocab) * D, rc, "t5.shared.weight");
-  h->t5.resize(cfg->t5_layers);
-  for (int i = 0; i < cfg->t5_layers; ++i) {
-    T5Layer& L = h->t5[i];
-    const std::string p = "t5.encoder.block." + std::to_string(i) + ".layer.";
-    L.qkv = take(h, static_cast<int64_t>(3) * I * D, rc);
-    alias(h, p + "0.SelfAttention.q.weight", L.qkv, static_cast<int64_t>(I) * D);
-    alias(h, p + "0.SelfAttention.k.weight", L.qkv + static_cast<int64_t>(I) * D, static_cast<int64_t>(I) * D);
-    alias(h, p + "0.SelfAttention.v.weight", L.qkv + static_cast<int64_t>(2) * I * D, static_cast<int64_t>(I) * D);
-    L.o = take(h, static_cast<int64_t>(D) * I, rc, p + "0.SelfAttention.o.weight");
-    L.ln0 = take(h, D, rc, p + "0.layer_norm.weight");
-    L.wi0 = take(h, static_cast<int64_t>(F) * D, rc, p + "1.DenseReluDense.wi_0.weight");
-    L.wi1 = take(h, static_cast<int64_t>(F) * D, rc, p + "1.DenseReluDense.wi_1.weight");
-    L.wo = take(h, static_cast<int64_t>(D) * F, rc, p + "1.DenseReluDense.wo.weight");
-    L.ln1 = take(h, D, rc, p + "1.layer_norm.weight");
-  }
-  h->t5_final = take(h, D, rc, "t5.encoder.final_layer_norm.weight");
-  const int C = cfg->clip_d_model;
-  h->clip_tok = take(h, static_cast<int64_t>(cfg->clip_vocab) * C, rc, "clip.text_model.embeddings.token_embedding.weight");
-  h->clip_pos = take(h, static_cast<int64_t>(cfg->clip_max_pos) * C, rc, "clip.text_model.embeddings.position_embedding.weight");
-  h->clip.resize(cfg->clip_layers);
-  for (int i = 0; i < cfg->clip_layers; ++i) {
-    ClipLayer& L = h->clip[i];
-    const std::string p = "clip.text_model.encoder.layers." + std::to_string(i) + ".";
-    L.ln1w = take(h, C, rc, p + "layer_norm1.weight");
-    L.ln1b = take(h, C, rc, p + "layer_norm1.bias");
-    L.qkvw = take(h, static_cast<int64_t>(3) * C * C, rc);
-    L.qkvb = take(h, 3 * C, rc);
-    const char* nm[3] = {"q_proj", "k_proj", "v_proj"};
-    for (int j = 0; j < 3; ++j) {
-      alias(h, p + "self_attn." + nm[j] + ".weight", L.qkvw + static_cast<int64_t>(j) * C * C, static_cast<int64_t>(C) * C);
-      alias(h, p + "self_attn." + nm[j] + ".bias", L.qkvb + j * C, C);
-    }
-    L.ow = take(h, static_cast<int64_t>(C) * C, rc, p + "self_attn.out_proj.weight");
-    L.ob = take(h, C, rc, p + "self_attn.out_proj.bias");
-    L.ln2w = take(h, C, rc, p + "layer_norm2.weight");
-    L.ln2b = take(h, C, rc, p + "layer_norm2.bias");
-    L.fc1w = take(h, static_cast<int64_t>(4) * C * C, rc, p + "mlp.fc1.weight");
-    L.fc1b = take(h, 4 * C, rc, p + "mlp.fc1.bias");
-    L.fc2w = take(h, static_cast<int64_t>(4) * C * C, rc, p + "mlp.fc2.weight");
-    L.fc2b = take(h, C, rc, p + "mlp.fc2.bias");
-  }
-  h->clip_fw = take(h, C, rc, "clip.text_model.final_layer_norm.weight");
-  h->clip_fb = take(h, C, rc, "clip.text_model.final_layer_norm.bias");
-  h->ones = take(h, 4096, rc);
-  if (!rc) {
-    std::vector<uint16_t> one(4096, 0x3F80);
-    if (cudaMemcpy(h->ones, one.data(), 8192, cudaMemcpyHostToDevice) != cudaSuccess) rc = -2;
-  }
+  const int rc = build_weights(h);
   if (rc) {
     rf_text_destroy(h);
     return rc;
@@ -549,7 +525,7 @@ int rf_text_create(const rf_text_config* cfg, rf_text** out) {
 
 void rf_text_destroy(rf_text* h) {
   if (!h) return;
-  for (void* p : h->allocs) cudaFree(p);
+  h->mem.release_all();
   delete h;
 }
 
@@ -558,22 +534,12 @@ int rf_text_load_weight(rf_text* h, const char* key, const void* src, int64_t nu
     rf::set_error("rf_text_load_weight: null argument");
     return -1;
   }
-  auto it = h->slots.find(key);
-  if (it == h->slots.end()) {
-    rf::set_error(std::string("rf_text_load_weight: unknown key ") + key);
-    return -4;
-  }
-  if (it->second.numel != numel) {
-    rf::set_error(std::string("rf_text_load_weight: size mismatch for ") + key + ": got " +
-                  std::to_string(numel) + ", want " + std::to_string(it->second.numel));
-    return -4;
-  }
-  RF_CHECK_CUDA(cudaMemcpy(it->second.dst, src, static_cast<size_t>(numel) * 2, cudaMemcpyDeviceToDevice));
-  it->second.loaded = true;
-  return 0;
+  return h->weights.load("rf_text_load_weight", key, src, numel);
 }
 
-int rf_text_missing_weights(rf_text* h, const char* prefix) { return h ? missing(h, prefix ? prefix : "") : -1; }
+int rf_text_missing_weights(rf_text* h, const char* prefix) {
+  return h ? h->weights.missing(prefix ? prefix : "", "missing text-encoder weights") : -1;
+}
 
 int rf_t5_encode(rf_text* h, const int* ids, int batch, int seq, const void* position_bias, void* out,
                  void* stream) {
@@ -581,25 +547,25 @@ int rf_t5_encode(rf_text* h, const int* ids, int batch, int seq, const void* pos
     rf::set_error("rf_t5_encode: bad argument");
     return -1;
   }
-  if (missing(h, "t5.") != 0) return -4;
+  if (rf_text_missing_weights(h, "t5.") != 0) return -4;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const rf_text_config& c = h->cfg;
   const int D = c.t5_d_model, F = c.t5_d_ff, I = c.t5_heads * 64, T = batch * seq;
-  RF_TRYT(ensure_ws(h, T));
+  RF_TRY(ensure_ws(h, T));
   bf16* xo = static_cast<bf16*>(out);  // residual stream lives in the caller's output buffer
-  RF_TRYT(rf::text_embed_launch(ids, h->t5_shared, nullptr, xo, T, seq, D, s));
+  RF_TRY(rf::text_embed_launch(ids, h->t5_shared, nullptr, xo, T, seq, D, s));
   for (int i = 0; i < c.t5_layers; ++i) {
     const T5Layer& L = h->t5[i];
-    RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln0, nullptr, c.t5_eps, 0, s));
-    RF_TRYT(linear(rf::EPI_BIAS, h->xn, D, T, L.qkv, nullptr, h->qkv, 3 * I, 3 * I, D, nullptr, 0, nullptr, s));
-    RF_TRYT(small_attn(h->qkv, h->qkv + I, h->qkv + 2 * I, 3 * I, h->att, I, batch, seq, c.t5_heads,
-                       static_cast<const bf16*>(position_bias), 1.0f, 0, 0, s));
-    RF_TRYT(linear(rf::EPI_GATE_RES, h->att, I, T, L.o, nullptr, xo, D, D, I, xo, D, h->ones, s));
-    RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln1, nullptr, c.t5_eps, 0, s));
-    RF_TRYT(rf::t5_gated_gelu(h->xn, T, D, L.wi0, L.wi1, F, h->h0, h->h1, s));
-    RF_TRYT(linear(rf::EPI_GATE_RES, h->h0, F, T, L.wo, nullptr, xo, D, D, F, xo, D, h->ones, s));
+    RF_TRY(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln0, nullptr, c.t5_eps, 0, s));
+    RF_TRY(linear(rf::EPI_BIAS, h->xn, D, T, L.qkv, nullptr, h->qkv, 3 * I, 3 * I, D, nullptr, 0, nullptr, s));
+    RF_TRY(small_attn(h->qkv, h->qkv + I, h->qkv + 2 * I, 3 * I, h->att, I, batch, seq, c.t5_heads,
+                      static_cast<const bf16*>(position_bias), 1.0f, 0, 0, s));
+    RF_TRY(linear(rf::EPI_GATE_RES, h->att, I, T, L.o, nullptr, xo, D, D, I, xo, D, h->ones, s));
+    RF_TRY(rf::text_rownorm_launch(xo, h->xn, T, D, L.ln1, nullptr, c.t5_eps, 0, s));
+    RF_TRY(rf::t5_gated_gelu(h->xn, T, D, L.wi0, L.wi1, F, h->h0, h->h1, s));
+    RF_TRY(linear(rf::EPI_GATE_RES, h->h0, F, T, L.wo, nullptr, xo, D, D, F, xo, D, h->ones, s));
   }
-  RF_TRYT(rf::text_rownorm_launch(xo, h->xn, T, D, h->t5_final, nullptr, c.t5_eps, 0, s));
+  RF_TRY(rf::text_rownorm_launch(xo, h->xn, T, D, h->t5_final, nullptr, c.t5_eps, 0, s));
   RF_CHECK_CUDA(cudaMemcpyAsync(xo, h->xn, static_cast<size_t>(T) * D * 2, cudaMemcpyDeviceToDevice, s));
   return 0;
 }
@@ -610,26 +576,26 @@ int rf_clip_encode(rf_text* h, const int* ids, const int* eos_pos, int batch, in
     rf::set_error("rf_clip_encode: bad argument");
     return -1;
   }
-  if (missing(h, "clip.") != 0) return -4;
+  if (rf_text_missing_weights(h, "clip.") != 0) return -4;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const rf_text_config& c = h->cfg;
   const int C = c.clip_d_model, T = batch * seq;
-  RF_TRYT(ensure_ws(h, T));
+  RF_TRY(ensure_ws(h, T));
   bf16* x = h->x;
-  RF_TRYT(rf::text_embed_launch(ids, h->clip_tok, h->clip_pos, x, T, seq, C, s));
+  RF_TRY(rf::text_embed_launch(ids, h->clip_tok, h->clip_pos, x, T, seq, C, s));
   for (int i = 0; i < c.clip_layers; ++i) {
     const ClipLayer& L = h->clip[i];
-    RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, L.ln1w, L.ln1b, 1e-5f, 1, s));
-    RF_TRYT(linear(rf::EPI_BIAS, h->xn, C, T, L.qkvw, L.qkvb, h->qkv, 3 * C, 3 * C, C, nullptr, 0, nullptr, s));
-    RF_TRYT(small_attn(h->qkv, h->qkv + C, h->qkv + 2 * C, 3 * C, h->att, C, batch, seq, c.clip_heads, nullptr,
-                       0.125f, 1, 1, s));
-    RF_TRYT(linear(rf::EPI_GATE_RES, h->att, C, T, L.ow, L.ob, x, C, C, C, x, C, h->ones, s));
-    RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, L.ln2w, L.ln2b, 1e-5f, 1, s));
-    RF_TRYT(linear(rf::EPI_BIAS, h->xn, C, T, L.fc1w, L.fc1b, h->h0, 4 * C, 4 * C, C, nullptr, 0, nullptr, s));
-    RF_TRYT(rf::text_ewise_launch(h->h0, nullptr, h->h0, static_cast<int64_t>(T) * 4 * C, 1, s));
-    RF_TRYT(linear(rf::EPI_GATE_RES, h->h0, 4 * C, T, L.fc2w, L.fc2b, x, C, C, 4 * C, x, C, h->ones, s));
+    RF_TRY(rf::text_rownorm_launch(x, h->xn, T, C, L.ln1w, L.ln1b, 1e-5f, 1, s));
+    RF_TRY(linear(rf::EPI_BIAS, h->xn, C, T, L.qkvw, L.qkvb, h->qkv, 3 * C, 3 * C, C, nullptr, 0, nullptr, s));
+    RF_TRY(small_attn(h->qkv, h->qkv + C, h->qkv + 2 * C, 3 * C, h->att, C, batch, seq, c.clip_heads, nullptr,
+                      0.125f, 1, 1, s));
+    RF_TRY(linear(rf::EPI_GATE_RES, h->att, C, T, L.ow, L.ob, x, C, C, C, x, C, h->ones, s));
+    RF_TRY(rf::text_rownorm_launch(x, h->xn, T, C, L.ln2w, L.ln2b, 1e-5f, 1, s));
+    RF_TRY(linear(rf::EPI_BIAS, h->xn, C, T, L.fc1w, L.fc1b, h->h0, 4 * C, 4 * C, C, nullptr, 0, nullptr, s));
+    RF_TRY(rf::text_ewise_launch(h->h0, nullptr, h->h0, static_cast<int64_t>(T) * 4 * C, 1, s));
+    RF_TRY(linear(rf::EPI_GATE_RES, h->h0, 4 * C, T, L.fc2w, L.fc2b, x, C, C, 4 * C, x, C, h->ones, s));
   }
-  RF_TRYT(rf::text_rownorm_launch(x, h->xn, T, C, h->clip_fw, h->clip_fb, 1e-5f, 1, s));
+  RF_TRY(rf::text_rownorm_launch(x, h->xn, T, C, h->clip_fw, h->clip_fb, 1e-5f, 1, s));
   if (hidden_out)
     RF_CHECK_CUDA(cudaMemcpyAsync(hidden_out, h->xn, static_cast<size_t>(T) * C * 2, cudaMemcpyDeviceToDevice, s));
   return rf::text_gather_rows_launch(h->xn, eos_pos, static_cast<bf16*>(pooled_out), batch, seq, C, s);

@@ -13,7 +13,6 @@
 #include <cmath>
 #include <cstring>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/rf_b200.h"
@@ -470,12 +469,10 @@ struct ConvW {
   bf16* w = nullptr;   // repacked [Cout_pad, taps * Cin_pad]
   bf16* b = nullptr;   // [Cout_pad]
   int cin = 0, cout = 0, cin_pad = 0, cout_pad = 0, taps = 9;
-  bool w_loaded = false, b_loaded = false;
 };
 struct Norm {
   bf16 *g = nullptr, *b = nullptr;
   int c = 0;
-  bool g_loaded = false, b_loaded = false;
 };
 struct Resnet {
   Norm n1, n2;
@@ -484,13 +481,9 @@ struct Resnet {
 };
 struct LinearW {
   bf16 *w = nullptr, *b = nullptr;
-  int out = 0, in = 0;
-  bool w_loaded = false, b_loaded = false;
 };
 }  // namespace
 
-extern "C" int rf_vae_missing_weights(struct rf_vae* h);
-static int vae_missing(struct rf_vae* h, const char* prefix);
 struct MidBlock {
   Resnet res[2];
   Norm attn_gn;
@@ -498,7 +491,9 @@ struct MidBlock {
 };
 
 struct rf_vae {
-  std::vector<void*> allocs;
+  rf::DeviceAllocs mem;     // weights, GroupNorm scratch, ones: live until destroy
+  rf::DeviceAllocs ws_mem;  // the size-dependent workspace below
+  rf::WeightTable weights;
   ConvW conv_in, conv_out;
   Norm norm_out;
   MidBlock mid;
@@ -510,8 +505,6 @@ struct rf_vae {
   MidBlock e_mid;
   Resnet down[4][2];
   ConvW downconv[3];
-  struct Slot { int kind; void* obj; int part; };  // kind 0 conv w, 1 conv b, 2 norm g, 3 norm b, 4 lin w, 5 lin b
-  std::unordered_map<std::string, Slot> slots;
   bf16* ones = nullptr;
   // workspace (sized for max_hw at first decode)
   int ws_h = 0, ws_w = 0;
@@ -522,7 +515,7 @@ struct rf_vae {
   float* gn_mr = nullptr;
   // ---- captured graphs: one decode / encode = ~150 launches whose tensor maps are encoded on the host, which made
   // the call host-bound (22 ms for 16 ms of kernels at 1024x1024).  The launch sequence of a geometry is captured
-  // once on `own_stream` against staging buffers and replayed; RF_VAE_GRAPH=0 and profiling runs stay eager.
+  // once on the side stream against staging buffers and replayed; RF_VAE_GRAPH=0 and profiling runs stay eager.
   struct Graph {
     int kind, height, width;            // kind 0 decode, 1 encode
     float scale, shift;
@@ -532,8 +525,7 @@ struct rf_vae {
     int64_t launches;
   };
   std::vector<Graph> graphs;
-  cudaStream_t own_stream = nullptr;    // capture is illegal on the legacy default stream
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
+  rf::SideStream side;
   uint8_t* g_u8 = nullptr;              // [H, W, 3] image staging (decode output / encode input)
   bf16* g_chw = nullptr;                // [3, H, W]
   bf16* g_lat = nullptr;                // packed latents [(H/16)(W/16), 64]
@@ -542,67 +534,52 @@ struct rf_vae {
 
 namespace {
 
-#define RF_TRYV(expr)           \
-  do {                          \
-    int _rc = (expr);           \
-    if (_rc != 0) return _rc;   \
-  } while (0)
-
-int valloc(rf_vae* h, void** p, size_t bytes) {
-  RF_CHECK_CUDA(cudaMalloc(p, bytes ? bytes : 16));
-  h->allocs.push_back(*p);
-  return 0;
-}
 int make_conv(rf_vae* h, ConvW& c, const std::string& key, int cin, int cout, int taps) {
   c.cin = cin; c.cout = cout; c.taps = taps;
   c.cin_pad = (cin + 63) / 64 * 64;
   c.cout_pad = (cout + 127) / 128 * 128;
-  void* p;
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(c.cout_pad) * taps * c.cin_pad * 2));
-  c.w = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(c.cout_pad) * 2));
-  c.b = static_cast<bf16*>(p);
+  RF_TRY(h->mem.alloc(&c.w, static_cast<size_t>(c.cout_pad) * taps * c.cin_pad));
+  RF_TRY(h->mem.alloc(&c.b, c.cout_pad));
   RF_CHECK_CUDA(cudaMemset(c.b, 0, static_cast<size_t>(c.cout_pad) * 2));
-  h->slots[key + ".weight"] = {0, &c, 0};
-  h->slots[key + ".bias"] = {1, &c, 0};
+  h->weights.add(key + ".weight", c.w, static_cast<int64_t>(cout) * cin * taps,
+                 rf::ConvRepack{cout, cin, taps, c.cout_pad, c.cin_pad});
+  h->weights.add(key + ".bias", c.b, cout);
   return 0;
 }
 int make_norm(rf_vae* h, Norm& n, const std::string& key, int c) {
   n.c = c;
-  void* p;
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(c) * 2)); n.g = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(c) * 2)); n.b = static_cast<bf16*>(p);
-  h->slots[key + ".weight"] = {2, &n, 0};
-  h->slots[key + ".bias"] = {3, &n, 0};
+  RF_TRY(h->mem.alloc(&n.g, c));
+  RF_TRY(h->mem.alloc(&n.b, c));
+  h->weights.add(key + ".weight", n.g, c);
+  h->weights.add(key + ".bias", n.b, c);
   return 0;
 }
 int make_resnet(rf_vae* h, Resnet& r, const std::string& key, int cin, int cout) {
-  RF_TRYV(make_norm(h, r.n1, key + ".norm1", cin));
-  RF_TRYV(make_conv(h, r.c1, key + ".conv1", cin, cout, 9));
-  RF_TRYV(make_norm(h, r.n2, key + ".norm2", cout));
-  RF_TRYV(make_conv(h, r.c2, key + ".conv2", cout, cout, 9));
+  RF_TRY(make_norm(h, r.n1, key + ".norm1", cin));
+  RF_TRY(make_conv(h, r.c1, key + ".conv1", cin, cout, 9));
+  RF_TRY(make_norm(h, r.n2, key + ".norm2", cout));
+  RF_TRY(make_conv(h, r.c2, key + ".conv2", cout, cout, 9));
   r.has_sc = cin != cout;
-  if (r.has_sc) RF_TRYV(make_conv(h, r.sc, key + ".conv_shortcut", cin, cout, 1));
+  if (r.has_sc) RF_TRY(make_conv(h, r.sc, key + ".conv_shortcut", cin, cout, 1));
   return 0;
 }
 
 int make_mid(rf_vae* h, MidBlock& m, const std::string& key) {
-  RF_TRYV(make_resnet(h, m.res[0], key + ".resnets.0", 512, 512));
-  RF_TRYV(make_resnet(h, m.res[1], key + ".resnets.1", 512, 512));
-  RF_TRYV(make_norm(h, m.attn_gn, key + ".attentions.0.group_norm", 512));
-  void* p;
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(1536) * 512 * 2)); m.attn_qkv.w = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, 1536 * 2)); m.attn_qkv.b = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, static_cast<size_t>(512) * 512 * 2)); m.attn_out.w = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, 512 * 2)); m.attn_out.b = static_cast<bf16*>(p);
+  RF_TRY(make_resnet(h, m.res[0], key + ".resnets.0", 512, 512));
+  RF_TRY(make_resnet(h, m.res[1], key + ".resnets.1", 512, 512));
+  RF_TRY(make_norm(h, m.attn_gn, key + ".attentions.0.group_norm", 512));
+  RF_TRY(h->mem.alloc(&m.attn_qkv.w, static_cast<size_t>(1536) * 512));
+  RF_TRY(h->mem.alloc(&m.attn_qkv.b, 1536));
+  RF_TRY(h->mem.alloc(&m.attn_out.w, static_cast<size_t>(512) * 512));
+  RF_TRY(h->mem.alloc(&m.attn_out.b, 512));
+  const std::string a = key + ".attentions.0.";
   const char* nm[3] = {"to_q", "to_k", "to_v"};
-  for (int j = 0; j < 3; ++j) {
-    const std::string k = key + ".attentions.0." + nm[j];
-    h->slots[k + ".weight"] = {4, &m.attn_qkv, j};
-    h->slots[k + ".bias"] = {5, &m.attn_qkv, j};
+  for (int j = 0; j < 3; ++j) {  // row slices of the stacked q | k | v projection
+    h->weights.add(a + nm[j] + ".weight", m.attn_qkv.w + j * 512 * 512, 512 * 512);
+    h->weights.add(a + nm[j] + ".bias", m.attn_qkv.b + j * 512, 512);
   }
-  h->slots[key + ".attentions.0.to_out.0.weight"] = {4, &m.attn_out, 3};
-  h->slots[key + ".attentions.0.to_out.0.bias"] = {5, &m.attn_out, 3};
+  h->weights.add(a + "to_out.0.weight", m.attn_out.w, 512 * 512);
+  h->weights.add(a + "to_out.0.bias", m.attn_out.b, 512);
   return 0;
 }
 
@@ -625,16 +602,6 @@ void drop_graphs(rf_vae* h) {
   h->graphs.clear();
 }
 
-void vfree(rf_vae* h, void* p) {
-  if (!p) return;
-  for (size_t i = 0; i < h->allocs.size(); ++i)
-    if (h->allocs[i] == p) {
-      h->allocs.erase(h->allocs.begin() + i);
-      break;
-    }
-  cudaFree(p);
-}
-
 // Every workspace size grows with the image height and width, so a workspace for (ws_h, ws_w) serves any
 // image that fits inside both.  A larger request grows it to the larger of each side (a 1024x1024 call after a
 // 768x1344 one makes room for 1024x1344), so alternating shapes allocate once, and frees the old one.
@@ -644,48 +611,30 @@ int ensure_workspace(rf_vae* h, int H, int W) {  // H, W: output image size
   if (H < h->ws_h) H = h->ws_h;
   if (W < h->ws_w) W = h->ws_w;
   if (h->buf[0]) RF_CHECK_CUDA(cudaDeviceSynchronize());  // work still queued on the old buffers
-  void** old[] = {reinterpret_cast<void**>(&h->g_u8), reinterpret_cast<void**>(&h->g_chw),
-                  reinterpret_cast<void**>(&h->g_lat), reinterpret_cast<void**>(&h->g_eps),
-                  reinterpret_cast<void**>(&h->buf[0]), reinterpret_cast<void**>(&h->buf[1]),
-                  reinterpret_cast<void**>(&h->buf[2]), reinterpret_cast<void**>(&h->buf[3]),
-                  reinterpret_cast<void**>(&h->tok), reinterpret_cast<void**>(&h->tokx),
-                  reinterpret_cast<void**>(&h->qkv), reinterpret_cast<void**>(&h->S),
-                  reinterpret_cast<void**>(&h->vt), reinterpret_cast<void**>(&h->ao),
-                  reinterpret_cast<void**>(&h->ay)};
-  for (void** q : old) {
-    vfree(h, *q);
-    *q = nullptr;
-  }
+  h->ws_mem.release_all();
   h->ws_h = h->ws_w = 0;  // stays 0 if an allocation below fails: the next call starts over
   for (int i = 0; i < 4; ++i) h->tag[i] = -1;
   const int lh = H / 8, lw = W / 8;
-  {
-    void* q;
-    RF_TRYV(valloc(h, &q, static_cast<size_t>(H) * W * 3)); h->g_u8 = static_cast<uint8_t*>(q);
-    RF_TRYV(valloc(h, &q, static_cast<size_t>(H) * W * 3 * 2)); h->g_chw = static_cast<bf16*>(q);
-    RF_TRYV(valloc(h, &q, static_cast<size_t>(H / 16) * (W / 16) * 64 * 2)); h->g_lat = static_cast<bf16*>(q);
-    RF_TRYV(valloc(h, &q, static_cast<size_t>(lh) * lw * 16 * 2)); h->g_eps = static_cast<bf16*>(q);
-  }
+  rf::DeviceAllocs& m = h->ws_mem;
+  RF_TRY(m.alloc(&h->g_u8, static_cast<size_t>(H) * W * 3));
+  RF_TRY(m.alloc(&h->g_chw, static_cast<size_t>(H) * W * 3));
+  RF_TRY(m.alloc(&h->g_lat, static_cast<size_t>(H / 16) * (W / 16) * 64));
+  RF_TRY(m.alloc(&h->g_eps, static_cast<size_t>(lh) * lw * 16));
   // largest padded tensor: full resolution x 256 channels (input of up_blocks.2's upsampler conv)
-  const size_t big = padded_elems(H, W, 256);
-  void* p;
-  for (int i = 0; i < 4; ++i) {
-    RF_TRYV(valloc(h, &p, big * 2));
-    h->buf[i] = static_cast<bf16*>(p);
-  }
+  for (int i = 0; i < 4; ++i) RF_TRY(m.alloc(&h->buf[i], padded_elems(H, W, 256)));
   // mid-block attention (decoder at H/8 x W/8; the encoder's is the same size): qkv, the staged K (ay) and V^T
   // run to the padded key count
   const size_t ntok = static_cast<size_t>(lh) * lw, npad = padded_tokens(lh, lw);
-  RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->tok = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->tokx = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, npad * 1536 * 2)); h->qkv = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * npad * 2)); h->S = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, npad * 512 * 2)); h->vt = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, ntok * 512 * 2)); h->ao = static_cast<bf16*>(p);
-  RF_TRYV(valloc(h, &p, npad * 512 * 2)); h->ay = static_cast<bf16*>(p);
+  RF_TRY(m.alloc(&h->tok, ntok * 512));
+  RF_TRY(m.alloc(&h->tokx, ntok * 512));
+  RF_TRY(m.alloc(&h->qkv, npad * 1536));
+  RF_TRY(m.alloc(&h->S, ntok * npad));
+  RF_TRY(m.alloc(&h->vt, npad * 512));
+  RF_TRY(m.alloc(&h->ao, ntok * 512));
+  RF_TRY(m.alloc(&h->ay, npad * 512));
   if (!h->gn_acc) {
-    RF_TRYV(valloc(h, &p, sizeof(float) * rf::gn_part_floats)); h->gn_acc = static_cast<float*>(p);
-    RF_TRYV(valloc(h, &p, sizeof(float) * 64)); h->gn_mr = static_cast<float*>(p);
+    RF_TRY(h->mem.alloc(&h->gn_acc, rf::gn_part_floats));
+    RF_TRY(h->mem.alloc(&h->gn_mr, 64));
   }
   h->ws_h = H; h->ws_w = W;
   return 0;
@@ -703,16 +652,16 @@ int prep(rf_vae* h, int i, int H, int W, int C, cudaStream_t s) {
 // ResnetBlock2D: buf[x] -> buf[out], scratch buf[t1], buf[t2]
 int resnet(rf_vae* h, const Resnet& r, int x, int out, int t1, int t2, int H, int W, cudaStream_t s) {
   const int cin = r.c1.cin_pad, cout = r.c1.cout_pad;
-  RF_TRYV(prep(h, t1, H, W, cin, s));
-  RF_TRYV(group_norm(h, h->buf[x], h->buf[t1], H, W, r.n1, 1, 1, 1, s));
-  RF_TRYV(prep(h, t2, H, W, cout, s));
-  RF_TRYV(conv(h, r.c1, h->buf[t1], h->buf[t2], nullptr, H, W, s));
-  RF_TRYV(prep(h, t1, H, W, cout, s));
-  RF_TRYV(group_norm(h, h->buf[t2], h->buf[t1], H, W, r.n2, 1, 1, 1, s));
-  RF_TRYV(prep(h, out, H, W, cout, s));
+  RF_TRY(prep(h, t1, H, W, cin, s));
+  RF_TRY(group_norm(h, h->buf[x], h->buf[t1], H, W, r.n1, 1, 1, 1, s));
+  RF_TRY(prep(h, t2, H, W, cout, s));
+  RF_TRY(conv(h, r.c1, h->buf[t1], h->buf[t2], nullptr, H, W, s));
+  RF_TRY(prep(h, t1, H, W, cout, s));
+  RF_TRY(group_norm(h, h->buf[t2], h->buf[t1], H, W, r.n2, 1, 1, 1, s));
+  RF_TRY(prep(h, out, H, W, cout, s));
   const bf16* shortcut = h->buf[x];
   if (r.has_sc) {
-    RF_TRYV(conv(h, r.sc, h->buf[x], h->buf[out], nullptr, H, W, s));  // 1x1 shortcut, into `out`
+    RF_TRY(conv(h, r.sc, h->buf[x], h->buf[out], nullptr, H, W, s));  // 1x1 shortcut, into `out`
     shortcut = h->buf[out];
   }
   // out = shortcut + conv2(t1): each residual box is read before the same box is stored (in place ok)
@@ -724,14 +673,14 @@ int resnet(rf_vae* h, const Resnet& r, int x, int out, int t1, int t2, int H, in
 // probability 0, so the padding changes no result.  With ntok % 128 == 0 there is no padding.
 int mid_attention(rf_vae* h, const MidBlock& m, const bf16* x, bf16* out, int H, int W, cudaStream_t s) {
   const int ntok = H * W, npad = padded_tokens(H, W);
-  RF_TRYV(rf::group_norm_launch(x, h->tok, H, W, 512, m.attn_gn.g, m.attn_gn.b, 0, 1, 0, h->gn_acc, h->gn_mr,
+  RF_TRY(rf::group_norm_launch(x, h->tok, H, W, 512, m.attn_gn.g, m.attn_gn.b, 0, 1, 0, h->gn_acc, h->gn_mr,
                                 s));  // compact tokens
-  RF_TRYV(rf::repad_launch(x, h->tokx, H, W, 512, 1, 0, s));
+  RF_TRY(rf::repad_launch(x, h->tokx, H, W, 512, 1, 0, s));
   rf::GemmGroupArgs g;
   memset(&g, 0, sizeof(g));  // q | k | v
   g.A = h->tok; g.lda = 512; g.M = ntok; g.W = m.attn_qkv.w; g.bias = m.attn_qkv.b;
   g.out = h->qkv; g.ldo = 1536;
-  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 1536, 512, 1, &g, s));
+  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, 1536, 512, 1, &g, s));
   // q | k | v rows of the padding keys (the GEMM writes rows [0, ntok) only)
   if (npad > ntok)
     RF_CHECK_CUDA(cudaMemsetAsync(h->qkv + static_cast<size_t>(ntok) * 1536, 0,
@@ -741,27 +690,27 @@ int mid_attention(rf_vae* h, const MidBlock& m, const bf16* x, bf16* out, int H,
                                   cudaMemcpyDeviceToDevice, s));
   memset(&g, 0, sizeof(g));  // S = Q K^T  [ntok, npad]
   g.A = h->qkv; g.lda = 1536; g.M = ntok; g.W = h->ay; g.out = h->S; g.ldo = npad;
-  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, npad, 512, 1, &g, s));
-  RF_TRYV(rf::softmax_rows_launch(h->S, ntok, npad, ntok, 1.0f / sqrtf(512.0f), s));
-  RF_TRYV(rf::transpose_launch(h->qkv + 1024, 1536, h->vt, npad, 512, s));  // V^T [512, npad]
+  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, npad, 512, 1, &g, s));
+  RF_TRY(rf::softmax_rows_launch(h->S, ntok, npad, ntok, 1.0f / sqrtf(512.0f), s));
+  RF_TRY(rf::transpose_launch(h->qkv + 1024, 1536, h->vt, npad, 512, s));  // V^T [512, npad]
   memset(&g, 0, sizeof(g));  // O = P V
   g.A = h->S; g.lda = npad; g.M = ntok; g.W = h->vt; g.out = h->ao; g.ldo = 512;
-  RF_TRYV(rf::gemm_launch(rf::EPI_BIAS, 512, npad, 1, &g, s));
+  RF_TRY(rf::gemm_launch(rf::EPI_BIAS, 512, npad, 1, &g, s));
   memset(&g, 0, sizeof(g));  // y = x + to_out(O)
   g.A = h->ao; g.lda = 512; g.M = ntok; g.W = m.attn_out.w; g.bias = m.attn_out.b;
   g.out = h->ay; g.ldo = 512; g.res = h->tokx; g.ldr = 512; g.gate = h->ones;
-  RF_TRYV(rf::gemm_launch(rf::EPI_GATE_RES, 512, 512, 1, &g, s));
+  RF_TRY(rf::gemm_launch(rf::EPI_GATE_RES, 512, 512, 1, &g, s));
   return rf::repad_launch(h->ay, out, H, W, 512, 0, 1, s);
 }
 
 // UNetMidBlock2D: resnet, self-attention, resnet.  buf[x] -> buf[x].
 int mid_block(rf_vae* h, const MidBlock& m, int& x, int& y, int t1, int t2, int H, int W, cudaStream_t s) {
-  RF_TRYV(resnet(h, m.res[0], x, y, t1, t2, H, W, s));
+  RF_TRY(resnet(h, m.res[0], x, y, t1, t2, H, W, s));
   std::swap(x, y);
-  RF_TRYV(prep(h, y, H, W, 512, s));
-  RF_TRYV(mid_attention(h, m, h->buf[x], h->buf[y], H, W, s));
+  RF_TRY(prep(h, y, H, W, 512, s));
+  RF_TRY(mid_attention(h, m, h->buf[x], h->buf[y], H, W, s));
   std::swap(x, y);
-  RF_TRYV(resnet(h, m.res[1], x, y, t1, t2, H, W, s));
+  RF_TRY(resnet(h, m.res[1], x, y, t1, t2, H, W, s));
   std::swap(x, y);
   return 0;
 }
@@ -782,23 +731,10 @@ bool use_graphs() {
   const char* e = getenv("RF_VAE_GRAPH");
   return !(e && atoi(e) == 0) && !rf::prof_on();
 }
-// work stream of the graph path: the caller's work is ordered before it by an event
-int graph_stream(rf_vae* h, cudaStream_t caller, cudaStream_t* s) {
-  if (!h->own_stream) {
-    RF_CHECK_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-    RF_CHECK_CUDA(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
-  }
-  RF_CHECK_CUDA(cudaEventRecord(h->ev_in, caller));
-  RF_CHECK_CUDA(cudaStreamWaitEvent(h->own_stream, h->ev_in, 0));
-  *s = h->own_stream;
-  return 0;
-}
 // replay the graph of (kind, geometry, factors, flags), capturing `body` first if it does not exist yet.  The
 // capture starts from "no zero ring valid", so a replay re-establishes every ring it relies on, whatever ran before.
-template <typename Body>
 int run_graph(rf_vae* h, int kind, int height, int width, float scale, float shift, int flags, cudaStream_t s,
-              Body&& body) {
+              const std::function<int()>& body) {
   rf_vae::Graph* g = nullptr;
   for (auto& c : h->graphs)
     if (c.kind == kind && c.height == height && c.width == width && c.scale == scale && c.shift == shift &&
@@ -806,30 +742,11 @@ int run_graph(rf_vae* h, int kind, int height, int width, float scale, float shi
       g = &c;
   if (!g) {
     for (int i = 0; i < 4; ++i) h->tag[i] = -1;
-    cudaGraph_t graph = nullptr;
-    const int64_t before = rf::launch_count();
-    RF_CHECK_CUDA(cudaStreamSynchronize(s));
-    RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int erc = body();
-    cudaError_t ce = cudaStreamEndCapture(s, &graph);
-    const int64_t launches = rf::launch_count() - before;
-    rf::count_launch(static_cast<int>(-launches));  // captured, not executed
-    if (erc || ce != cudaSuccess) {
-      if (graph) cudaGraphDestroy(graph);
+    rf_vae::Graph ng{kind, height, width, scale, shift, flags, nullptr, {0, 0, 0, 0}, 0};
+    const int rc = rf::capture_graph(s, "rf_vae", body, &ng.exec, &ng.launches);
+    if (rc) {
       for (int i = 0; i < 4; ++i) h->tag[i] = -1;
-      if (!erc) {
-        rf::set_error(std::string("rf_vae: graph capture failed: ") + cudaGetErrorString(ce));
-        erc = -2;
-      }
-      return erc;
-    }
-    rf_vae::Graph ng{kind, height, width, scale, shift, flags, nullptr, {0, 0, 0, 0}, launches};
-    ce = cudaGraphInstantiate(&ng.exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) {
-      for (int i = 0; i < 4; ++i) h->tag[i] = -1;
-      rf::set_error(std::string("rf_vae: cudaGraphInstantiate: ") + cudaGetErrorString(ce));
-      return -2;
+      return rc;
     }
     for (int i = 0; i < 4; ++i) ng.tag_end[i] = h->tag[i];
     if (h->graphs.size() >= 8) {  // a handful of geometries in practice (decode 1024, encode 512)
@@ -860,11 +777,7 @@ int rf_vae_create(rf_vae** out) {
     rf::set_error("rf_vae_create: null argument");
     return -1;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    rf::set_error("rf_vae_create: no CUDA device (this library has no CPU fallback)");
-    return -3;
-  }
+  RF_TRY(rf::require_device("rf_vae_create"));
   rf_vae* h = new rf_vae();
   int rc = 0;
   auto chk = [&](int r) { if (r && !rc) rc = r; };
@@ -903,13 +816,9 @@ int rf_vae_create(rf_vae** out) {
   chk(make_mid(h, h->e_mid, "encoder.mid_block"));
   chk(make_norm(h, h->e_norm_out, "encoder.conv_norm_out", 512));
   chk(make_conv(h, h->e_conv_out, "encoder.conv_out", 512, 32, 9));
-  {
-    void* p;
-    chk(valloc(h, &p, 512 * 2));
-    h->ones = static_cast<bf16*>(p);
-    std::vector<uint16_t> one(512, 0x3F80);
-    if (!rc && cudaMemcpy(h->ones, one.data(), 1024, cudaMemcpyHostToDevice) != cudaSuccess) rc = -2;
-  }
+  chk(h->mem.alloc(&h->ones, 512));
+  const std::vector<uint16_t> one(512, 0x3F80);
+  if (!rc && cudaMemcpy(h->ones, one.data(), 1024, cudaMemcpyHostToDevice) != cudaSuccess) rc = -2;
   if (rc) {
     rf_vae_destroy(h);
     return rc;
@@ -921,10 +830,9 @@ int rf_vae_create(rf_vae** out) {
 void rf_vae_destroy(rf_vae* h) {
   if (!h) return;
   drop_graphs(h);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
-  if (h->ev_in) cudaEventDestroy(h->ev_in);
-  if (h->ev_out) cudaEventDestroy(h->ev_out);
-  for (void* p : h->allocs) cudaFree(p);
+  h->side.destroy();
+  h->ws_mem.release_all();
+  h->mem.release_all();
   delete h;
 }
 
@@ -933,46 +841,7 @@ int rf_vae_load_weight(rf_vae* h, const char* key, const void* src, int64_t nume
     rf::set_error("rf_vae_load_weight: null argument");
     return -1;
   }
-  auto it = h->slots.find(key);
-  if (it == h->slots.end()) {
-    rf::set_error(std::string("rf_vae_load_weight: unknown key ") + key);
-    return -4;
-  }
-  const rf_vae::Slot& sl = it->second;
-  const bf16* s = static_cast<const bf16*>(src);
-  auto bad = [&](int64_t want) {
-    rf::set_error(std::string("rf_vae_load_weight: size mismatch for ") + key + ": got " +
-                  std::to_string(numel) + ", want " + std::to_string(want));
-    return -4;
-  };
-  if (sl.kind == 0) {
-    ConvW& c = *static_cast<ConvW*>(sl.obj);
-    if (numel != static_cast<int64_t>(c.cout) * c.cin * c.taps) return bad(static_cast<int64_t>(c.cout) * c.cin * c.taps);
-    RF_TRYV(rf::conv_repack_launch(s, c.w, c.cout, c.cin, c.taps, c.cout_pad, c.cin_pad, nullptr));
-    c.w_loaded = true;
-  } else if (sl.kind == 1) {
-    ConvW& c = *static_cast<ConvW*>(sl.obj);
-    if (numel != c.cout) return bad(c.cout);
-    RF_CHECK_CUDA(cudaMemcpy(c.b, s, static_cast<size_t>(c.cout) * 2, cudaMemcpyDeviceToDevice));
-    c.b_loaded = true;
-  } else if (sl.kind == 2 || sl.kind == 3) {
-    Norm& n = *static_cast<Norm*>(sl.obj);
-    if (numel != n.c) return bad(n.c);
-    RF_CHECK_CUDA(cudaMemcpy(sl.kind == 2 ? n.g : n.b, s, static_cast<size_t>(n.c) * 2, cudaMemcpyDeviceToDevice));
-    (sl.kind == 2 ? n.g_loaded : n.b_loaded) = true;
-  } else {
-    LinearW& l = *static_cast<LinearW*>(sl.obj);
-    const int row0 = sl.part < 3 ? sl.part * 512 : 0;
-    if (sl.kind == 4) {
-      if (numel != 512 * 512) return bad(512 * 512);
-      RF_CHECK_CUDA(cudaMemcpy(l.w + static_cast<size_t>(row0) * 512, s, 512 * 512 * 2, cudaMemcpyDeviceToDevice));
-      l.w_loaded = true;
-    } else {
-      if (numel != 512) return bad(512);
-      RF_CHECK_CUDA(cudaMemcpy(l.b + row0, s, 512 * 2, cudaMemcpyDeviceToDevice));
-      l.b_loaded = true;
-    }
-  }
+  RF_TRY(h->weights.load("rf_vae_load_weight", key, src, numel));
   RF_CHECK_CUDA(cudaDeviceSynchronize());
   return 0;
 }
@@ -983,27 +852,25 @@ int rf_vae_decode(rf_vae* h, const void* packed_latents, int height, int width, 
     rf::set_error("rf_vae_decode: null argument");
     return -1;
   }
-  RF_TRYV(check_size("rf_vae_decode", height, width));
-  RF_TRYV(ensure_workspace(h, height, width));
-  if (vae_missing(h, "decoder.") != 0) return -4;
+  RF_TRY(check_size("rf_vae_decode", height, width));
+  RF_TRY(ensure_workspace(h, height, width));
+  if (h->weights.missing("decoder.", "missing VAE weights") != 0) return -4;
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
   if (!use_graphs()) return decode_body(h, packed_latents, height, width, scaling_factor, shift_factor, out_u8_hwc,
                                         out_bf16_chw, caller);
   cudaStream_t s = nullptr;
-  RF_TRYV(graph_stream(h, caller, &s));
+  RF_TRY(h->side.enter(caller, &s));
   const size_t lat_bytes = static_cast<size_t>(height / 16) * (width / 16) * 64 * 2;
   RF_CHECK_CUDA(cudaMemcpyAsync(h->g_lat, packed_latents, lat_bytes, cudaMemcpyDeviceToDevice, s));
   const int flags = (out_u8_hwc ? 1 : 0) | (out_bf16_chw ? 2 : 0);
-  RF_TRYV(run_graph(h, 0, height, width, scaling_factor, shift_factor, flags, s, [&]() {
+  RF_TRY(run_graph(h, 0, height, width, scaling_factor, shift_factor, flags, s, [&]() {
     return decode_body(h, h->g_lat, height, width, scaling_factor, shift_factor, out_u8_hwc ? h->g_u8 : nullptr,
                        out_bf16_chw ? h->g_chw : nullptr, s);
   }));
   const size_t px = static_cast<size_t>(height) * width * 3;
   if (out_u8_hwc) RF_CHECK_CUDA(cudaMemcpyAsync(out_u8_hwc, h->g_u8, px, cudaMemcpyDeviceToDevice, s));
   if (out_bf16_chw) RF_CHECK_CUDA(cudaMemcpyAsync(out_bf16_chw, h->g_chw, px * 2, cudaMemcpyDeviceToDevice, s));
-  RF_CHECK_CUDA(cudaEventRecord(h->ev_out, s));
-  RF_CHECK_CUDA(cudaStreamWaitEvent(caller, h->ev_out, 0));
-  return 0;
+  return h->side.leave(caller);
 }
 
 static int decode_body(rf_vae* h, const void* packed_latents, int height, int width, float scaling_factor,
@@ -1012,38 +879,38 @@ static int decode_body(rf_vae* h, const void* packed_latents, int height, int wi
   int x = 0, y = 1;
   const int t1 = 2, t2 = 3;
   // ---- latents -> NHWC (16 real channels of 64), conv_in
-  RF_TRYV(prep(h, x, H, W, 64, s));
-  RF_TRYV(rf::unpack_latents_launch(static_cast<const bf16*>(packed_latents), h->buf[x], H, W, scaling_factor,
-                                    shift_factor, s));
-  RF_TRYV(prep(h, y, H, W, 512, s));
-  RF_TRYV(conv(h, h->conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
+  RF_TRY(prep(h, x, H, W, 64, s));
+  RF_TRY(rf::unpack_latents_launch(static_cast<const bf16*>(packed_latents), h->buf[x], H, W, scaling_factor,
+                                   shift_factor, s));
+  RF_TRY(prep(h, y, H, W, 512, s));
+  RF_TRY(conv(h, h->conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
   std::swap(x, y);
-  RF_TRYV(mid_block(h, h->mid, x, y, t1, t2, H, W, s));  // result back in buf[x]
+  RF_TRY(mid_block(h, h->mid, x, y, t1, t2, H, W, s));  // result back in buf[x]
   // ---- up blocks: 3 resnets each, nearest 2x + conv between them
   for (int i = 0; i < 4; ++i) {
     for (int j = 0; j < 3; ++j) {
-      RF_TRYV(resnet(h, h->up[i][j], x, y, t1, t2, H, W, s));
+      RF_TRY(resnet(h, h->up[i][j], x, y, t1, t2, H, W, s));
       std::swap(x, y);
     }
     if (i < 3) {
       const int C = h->upconv[i].cin_pad;
-      RF_TRYV(prep(h, y, 2 * H, 2 * W, C, s));
-      RF_TRYV(rf::upsample2x_launch(h->buf[x], h->buf[y], H, W, C, s));
+      RF_TRY(prep(h, y, 2 * H, 2 * W, C, s));
+      RF_TRY(rf::upsample2x_launch(h->buf[x], h->buf[y], H, W, C, s));
       H *= 2;
       W *= 2;
-      RF_TRYV(prep(h, x, H, W, C, s));
-      RF_TRYV(conv(h, h->upconv[i], h->buf[y], h->buf[x], nullptr, H, W, s));
+      RF_TRY(prep(h, x, H, W, C, s));
+      RF_TRY(conv(h, h->upconv[i], h->buf[y], h->buf[x], nullptr, H, W, s));
     }
   }
   // ---- norm_out + SiLU + conv_out (3 channels padded to 128) + post-process
-  RF_TRYV(prep(h, t1, H, W, 128, s));
-  RF_TRYV(group_norm(h, h->buf[x], h->buf[t1], H, W, h->norm_out, 1, 1, 1, s));
-  RF_TRYV(prep(h, y, H, W, 128, s));
-  RF_TRYV(conv(h, h->conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));
+  RF_TRY(prep(h, t1, H, W, 128, s));
+  RF_TRY(group_norm(h, h->buf[x], h->buf[t1], H, W, h->norm_out, 1, 1, 1, s));
+  RF_TRY(prep(h, y, H, W, 128, s));
+  RF_TRY(conv(h, h->conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));
   return rf::postprocess_launch(h->buf[y], H, W, 128, out_u8_hwc, static_cast<bf16*>(out_bf16_chw), s);
 }
 
-int rf_vae_missing_weights(rf_vae* h) { return vae_missing(h, ""); }
+int rf_vae_missing_weights(rf_vae* h) { return h ? h->weights.missing("", "missing VAE weights") : -1; }
 
 }  // extern "C"
 
@@ -1052,8 +919,10 @@ int vae_mid_attention(rf_vae* h, int encoder, const bf16* x, bf16* out, int H, i
     rf::set_error("vae_mid_attention: null argument or latent size outside [1, 2048]");
     return -1;
   }
-  if (vae_missing(h, encoder ? "encoder.mid_block.attentions." : "decoder.mid_block.attentions.") != 0) return -4;
-  RF_TRYV(ensure_workspace(h, 8 * H, 8 * W));
+  if (h->weights.missing(encoder ? "encoder.mid_block.attentions." : "decoder.mid_block.attentions.",
+                         "missing VAE weights") != 0)
+    return -4;
+  RF_TRY(ensure_workspace(h, 8 * H, 8 * W));
   return mid_attention(h, encoder ? h->e_mid : h->mid, x, out, H, W, s);
 }
 
@@ -1069,29 +938,27 @@ int rf_vae_encode(rf_vae* h, const uint8_t* image_u8_hwc, const void* image_bf16
     rf::set_error("rf_vae_encode: null argument");
     return -1;
   }
-  RF_TRYV(check_size("rf_vae_encode", height, width));
-  RF_TRYV(ensure_workspace(h, height, width));
-  if (vae_missing(h, "encoder.") != 0) return -4;
+  RF_TRY(check_size("rf_vae_encode", height, width));
+  RF_TRY(ensure_workspace(h, height, width));
+  if (h->weights.missing("encoder.", "missing VAE weights") != 0) return -4;
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
   if (!use_graphs()) return encode_body(h, image_u8_hwc, image_bf16_chw, height, width, eps_bf16_chw, scaling_factor,
                                         shift_factor, packed_out, caller);
   cudaStream_t s = nullptr;
-  RF_TRYV(graph_stream(h, caller, &s));
+  RF_TRY(h->side.enter(caller, &s));
   const size_t px = static_cast<size_t>(height) * width * 3;
   if (image_u8_hwc) RF_CHECK_CUDA(cudaMemcpyAsync(h->g_u8, image_u8_hwc, px, cudaMemcpyDeviceToDevice, s));
   else RF_CHECK_CUDA(cudaMemcpyAsync(h->g_chw, image_bf16_chw, px * 2, cudaMemcpyDeviceToDevice, s));
   const size_t eps_bytes = static_cast<size_t>(height / 8) * (width / 8) * 16 * 2;
   if (eps_bf16_chw) RF_CHECK_CUDA(cudaMemcpyAsync(h->g_eps, eps_bf16_chw, eps_bytes, cudaMemcpyDeviceToDevice, s));
   const int flags = (image_u8_hwc ? 1 : 2) | (eps_bf16_chw ? 4 : 0);
-  RF_TRYV(run_graph(h, 1, height, width, scaling_factor, shift_factor, flags, s, [&]() {
+  RF_TRY(run_graph(h, 1, height, width, scaling_factor, shift_factor, flags, s, [&]() {
     return encode_body(h, image_u8_hwc ? h->g_u8 : nullptr, image_u8_hwc ? nullptr : h->g_chw, height, width,
                        eps_bf16_chw ? h->g_eps : nullptr, scaling_factor, shift_factor, h->g_lat, s);
   }));
   RF_CHECK_CUDA(cudaMemcpyAsync(packed_out, h->g_lat, static_cast<size_t>(height / 16) * (width / 16) * 64 * 2,
                                 cudaMemcpyDeviceToDevice, s));
-  RF_CHECK_CUDA(cudaEventRecord(h->ev_out, s));
-  RF_CHECK_CUDA(cudaStreamWaitEvent(caller, h->ev_out, 0));
-  return 0;
+  return h->side.leave(caller);
 }
 
 static int encode_body(rf_vae* h, const uint8_t* image_u8_hwc, const void* image_bf16_chw, int height, int width,
@@ -1100,57 +967,33 @@ static int encode_body(rf_vae* h, const uint8_t* image_u8_hwc, const void* image
   int H = height, W = width;
   int x = 0, y = 1;
   const int t1 = 2, t2 = 3;
-  RF_TRYV(prep(h, x, H, W, 64, s));
-  RF_TRYV(rf::image_to_nhwc_launch(image_u8_hwc, static_cast<const bf16*>(image_bf16_chw), h->buf[x], H, W, s));
-  RF_TRYV(prep(h, y, H, W, 128, s));
-  RF_TRYV(conv(h, h->e_conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
+  RF_TRY(prep(h, x, H, W, 64, s));
+  RF_TRY(rf::image_to_nhwc_launch(image_u8_hwc, static_cast<const bf16*>(image_bf16_chw), h->buf[x], H, W, s));
+  RF_TRY(prep(h, y, H, W, 128, s));
+  RF_TRY(conv(h, h->e_conv_in, h->buf[x], h->buf[y], nullptr, H, W, s));
   std::swap(x, y);
   for (int i = 0; i < 4; ++i) {
     for (int j = 0; j < 2; ++j) {
-      RF_TRYV(resnet(h, h->down[i][j], x, y, t1, t2, H, W, s));
+      RF_TRY(resnet(h, h->down[i][j], x, y, t1, t2, H, W, s));
       std::swap(x, y);
     }
     if (i < 3) {  // Downsample2D: pad (0,1,0,1) + conv3x3 stride 2 == strided taps over the zero ring
       const ConvW& c = h->downconv[i];
       H /= 2;
       W /= 2;
-      RF_TRYV(prep(h, y, H, W, c.cout_pad, s));
-      RF_TRYV(rf::conv_launch(h->buf[x], c.w, c.b, h->buf[y], nullptr, h->ones, H, W, c.cin_pad,
-                              c.cout_pad, 9, 2, s));
+      RF_TRY(prep(h, y, H, W, c.cout_pad, s));
+      RF_TRY(rf::conv_launch(h->buf[x], c.w, c.b, h->buf[y], nullptr, h->ones, H, W, c.cin_pad,
+                             c.cout_pad, 9, 2, s));
       std::swap(x, y);
     }
   }
-  RF_TRYV(mid_block(h, h->e_mid, x, y, t1, t2, H, W, s));
-  RF_TRYV(prep(h, t1, H, W, 512, s));
-  RF_TRYV(group_norm(h, h->buf[x], h->buf[t1], H, W, h->e_norm_out, 1, 1, 1, s));
-  RF_TRYV(prep(h, y, H, W, 128, s));
-  RF_TRYV(conv(h, h->e_conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));  // 32 moments (of 128)
+  RF_TRY(mid_block(h, h->e_mid, x, y, t1, t2, H, W, s));
+  RF_TRY(prep(h, t1, H, W, 512, s));
+  RF_TRY(group_norm(h, h->buf[x], h->buf[t1], H, W, h->e_norm_out, 1, 1, 1, s));
+  RF_TRY(prep(h, y, H, W, 128, s));
+  RF_TRY(conv(h, h->e_conv_out, h->buf[t1], h->buf[y], nullptr, H, W, s));  // 32 moments (of 128)
   return rf::sample_pack_launch(h->buf[y], 128, static_cast<const bf16*>(eps_bf16_chw),
                                 static_cast<bf16*>(packed_out), H, W, scaling_factor, shift_factor, s);
 }
 
 }  // extern "C"
-
-static int vae_missing(rf_vae* h, const char* prefix) {
-  if (!h) return -1;
-  int missing = 0;
-  std::string names;
-  const size_t pl = strlen(prefix);
-  for (auto& kv : h->slots) {
-    if (kv.first.compare(0, pl, prefix) != 0) continue;
-    bool ok = true;
-    const rf_vae::Slot& sl = kv.second;
-    if (sl.kind == 0) ok = static_cast<ConvW*>(sl.obj)->w_loaded;
-    else if (sl.kind == 1) ok = static_cast<ConvW*>(sl.obj)->b_loaded;
-    else if (sl.kind == 2) ok = static_cast<Norm*>(sl.obj)->g_loaded;
-    else if (sl.kind == 3) ok = static_cast<Norm*>(sl.obj)->b_loaded;
-    else if (sl.kind == 4) ok = static_cast<LinearW*>(sl.obj)->w_loaded;
-    else ok = static_cast<LinearW*>(sl.obj)->b_loaded;
-    if (!ok) {
-      if (missing < 6) names += kv.first + " ";
-      ++missing;
-    }
-  }
-  if (missing) rf::set_error("missing VAE weights: " + names);
-  return missing;
-}

@@ -283,13 +283,16 @@ def _rewrite(src_dir, dst_dir, edit):
     return dst_dir
 
 
-@pytest.mark.parametrize("comp", ["transformer", "vae"])
-def test_strict_loading_names_the_key(ckpt, tmp_path, comp):
+@pytest.mark.parametrize("comp,gone", [
+    pytest.param("transformer", "single_transformer_blocks.1.proj_mlp.bias", id="transformer"),
+    pytest.param("vae", "decoder.up_blocks.2.resnets.1.conv2.weight", id="vae"),
+    # one row slice of the mid-block attention's stacked q | k | v projection
+    pytest.param("vae", "decoder.mid_block.attentions.0.to_k.weight", id="vae-mid-attention"),
+])
+def test_strict_loading_names_the_key(ckpt, tmp_path, comp, gone):
     from reflectionflow_b200.transformer import B200FluxTransformer2DModel
     from reflectionflow_b200.vae import B200AutoencoderKL
     src = os.path.join(ckpt["one"], comp)
-    gone = "single_transformer_blocks.1.proj_mlp.bias" if comp == "transformer" else \
-        "decoder.up_blocks.2.resnets.1.conv2.weight"
     extra = "transformer_blocks.0.attn.to_x.weight" if comp == "transformer" else "decoder.extra_block.weight"
     load = (lambda d: B200FluxTransformer2DModel.from_pretrained(d)) if comp == "transformer" else \
         (lambda d: B200AutoencoderKL.from_pretrained(d))
