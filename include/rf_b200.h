@@ -235,6 +235,34 @@ int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* tx
                                   float guidance_scale, const void* cond_latents, const void* uncond_latents,
                                   float image_guidance_scale, void* stream);
 
+/* The denoise loop one step at a time, for per-step callbacks (diffusers' callback_on_step_end, generate.py:283-290):
+ * step i runs for every sample before the caller sees the whole batch, and may then change the latents or the T5
+ * states before step i + 1.
+ *
+ * rf_dit_denoise_begin opens a session: it uploads the schedule (as rf_dit_denoise), builds every sample's
+ * modulation tables once (the step table of each sample at guidance_scale; with image guidance also the uncond
+ * table at guidance 1; with a condition stream the cond_temb table), stages cond_latents [B, n_cond, 64], and
+ * captures the step graph unless the one rf_dit_denoise / rf_dit_denoise_image_guidance would replay is current.
+ * image_guidance_scale != 1 (as fp32) opens an image-guided session (same needs as
+ * rf_dit_denoise_image_guidance).  pooled is only read here: it cannot change within a session.
+ *
+ * rf_dit_denoise_step runs step i for every sample, in place on latents_inout [B, n_img, 64], with txt
+ * [B, n_txt, 4096] as the text input; an image-guided session takes that step's uncond condition latents
+ * uncond_latents_i [B, n_cond, 64], an unguided one NULL.  Per sample it copies the latents, text, condition and
+ * U_i into the captured step's staging, copies the sample's table rows into the rows the step selects and the step
+ * index from device memory (no host-to-device copy), replays the graph and copies the latents back: no host
+ * synchronisation, no capture.  Steps may run in any order and repeat; running 0 .. n_steps-1 once each on
+ * unchanged inputs gives rf_dit_denoise's bytes.
+ *
+ * rf_dit_prepare, rf_dit_load_weight, rf_dit_set_lora, rf_dit_clear_lora, rf_dit_set_lora_scale, rf_dit_denoise,
+ * rf_dit_denoise_image_guidance and a new rf_dit_denoise_begin close the session; rf_dit_denoise_step then fails
+ * with a message.  rf_dit_forward leaves it open. */
+int rf_dit_denoise_begin(rf_dit* h, const void* pooled, const uint16_t* timesteps_bf16_host, const float* sigmas_host,
+                         int n_steps, float guidance_scale, const void* cond_latents, float image_guidance_scale,
+                         void* stream);
+int rf_dit_denoise_step(rf_dit* h, int i, void* latents_inout, const void* txt, const void* uncond_latents_i,
+                        void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * FLUX VAE decoder (next-tier row: `vae.decode` + `image_processor.postprocess`,
  * train_flux/flux/generate.py:302-307).
@@ -272,6 +300,8 @@ int rf_profile_stop(char* json_out, int capacity);
 
 /* number of kernels this library launched since process start (for bench.py's gpu_launches) */
 int64_t rf_launch_count(void);
+/* Number of CUDA graphs captured so far by every handle of the process (the DiT step, the VAE graphs). */
+int64_t rf_graph_capture_count(void);
 
 /* ---- text encoders (T5 encoder + CLIP text model) --------------------------------------------
  * Replaces `pipe.text_encoder_2(ids)[0]` and `pipe.text_encoder(ids).pooler_output` inside diffusers

@@ -27,6 +27,7 @@ def _declare(lib):
     lib.rf_last_error.argtypes = []
     lib.rf_abi_version.restype = ci
     lib.rf_launch_count.restype = c_int64
+    lib.rf_graph_capture_count.restype = c_int64
     lib.rf_profile_start.restype = ci
     lib.rf_profile_stop.restype = ci
     lib.rf_profile_stop.argtypes = [c_char_p, ci]
@@ -102,6 +103,10 @@ def _declare(lib):
         lib.rf_dit_denoise.argtypes = [vp, vp, vp, vp, vp, vp, ci, cf, vp, vp]
         lib.rf_dit_denoise_image_guidance.restype = ci
         lib.rf_dit_denoise_image_guidance.argtypes = [vp, vp, vp, vp, vp, vp, ci, cf, vp, vp, cf, vp]
+        lib.rf_dit_denoise_begin.restype = ci
+        lib.rf_dit_denoise_begin.argtypes = [vp, vp, vp, vp, ci, cf, vp, cf, vp]
+        lib.rf_dit_denoise_step.restype = ci
+        lib.rf_dit_denoise_step.argtypes = [vp, ci, vp, vp, vp, vp]
 
 
 def load():

@@ -151,6 +151,17 @@ struct rf_dit {
   int s_cap_steps_u = 0;
   StepGraph graph, graph_ig;  // the captured step of rf_dit_denoise / of the guided loop
   rf::SideStream side;        // the denoise loop's stream
+  // step-wise session (rf_dit_denoise_begin / rf_dit_denoise_step): every sample's tables, built once at begin.
+  // Before each replay of the captured step, sample b's row i is copied into the row the step selects
+  // (s_mod_all[i], s_mod_all_u[i]) and its cond_temb table into MODC.  Everything that drops the captured step or
+  // changes what the tables were built from closes the session (sess = false).
+  bool sess = false, sess_guided = false;
+  int sess_steps = 0;
+  int64_t sess_rows = 0, sess_rows_u = 0;  // rows of sess_mod / sess_mod_u (B x n_steps)
+  bf16 *sess_mod = nullptr, *sess_mod_u = nullptr;  // [B, n_steps, n_mod]
+  bf16 *sess_modc = nullptr, *sess_cond = nullptr;  // [B, n_mod] cond_temb tables, [B, n_cond, C] condition latents
+  int* sess_idx = nullptr;                          // 0, 1, ..., sess_idx_n - 1: the step index copied into s_step
+  int sess_idx_n = 0;
 };
 
 namespace {
@@ -439,8 +450,8 @@ int temb_mod(rf_dit* h, int n, const bf16* t, const bf16* guid, const bf16* pool
 
 // cond_temb and MODC: step-invariant (transformer.py:108-114 recomputes them every step).  t = c_t * 1000 = 0,
 // guidance = 1000 (s_zero_one = {bf16 0, bf16 1}); the condition rows read no norm1_context / norm_out section of MODC.
-int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s) {
-  return temb_mod(h, 1, h->s_zero_one, h->s_zero_one + 1, pooled, true, false, h->MODC, h->emb_ws, s);
+int compute_cond_mod(rf_dit* h, const bf16* pooled, cudaStream_t s, bf16* out = nullptr) {
+  return temb_mod(h, 1, h->s_zero_one, h->s_zero_one + 1, pooled, true, false, out ? out : h->MODC, h->emb_ws, s);
 }
 
 // some member of pack p adds a term (lora_on) / is set
@@ -738,6 +749,7 @@ int alloc_lora_ws(rf_dit* h, int rows) {
 bool merged_current(const rf_dit* h) { return h->lora_merged && h->merged_call_scale == h->call_scale; }
 
 void drop_graph(rf_dit* h) {
+  h->sess = false;  // the session replays this graph
   for (StepGraph* g : {&h->graph, &h->graph_ig}) {
     if (g->exec) {
       cudaGraphExecDestroy(g->exec);
@@ -755,6 +767,10 @@ void free_geometry(rf_dit* h) {
   h->s_sigmas = nullptr;
   h->s_cap_steps_u = 0;
   h->s_mod_all_u = nullptr;
+  h->sess_rows = h->sess_rows_u = 0;
+  h->sess_mod = h->sess_mod_u = h->sess_modc = h->sess_cond = nullptr;
+  h->sess_idx = nullptr;
+  h->sess_idx_n = 0;
 }
 
 }  // namespace
@@ -914,6 +930,7 @@ int rf_dit_load_weight(rf_dit* h, const char* key, const void* src, int64_t nume
   }
   RF_TRY(h->weights.load("rf_dit_load_weight", key, src, numel));
   h->lora_merged = false;  // merged W + BA copies (fuse_lora mode) are stale now
+  h->sess = false;         // and so are the session's modulation tables
   return 0;
 }
 
@@ -995,8 +1012,9 @@ int rf_dit_set_lora_scale(rf_dit* h, double scale) {
     return -1;
   }
   // takes effect at the next call: the merged copies are re-merged (check_ready) and the captured step is
-  // re-captured (rf_dit_denoise) when they were built for another scale
+  // re-captured (rf_dit_denoise) when they were built for another scale; the session's tables hold the old scale
   h->call_scale = scale;
+  h->sess = false;
   return 0;
 }
 
@@ -1186,17 +1204,10 @@ static int capture_step(rf_dit* h, bool guided, StepGraph* g, cudaStream_t s) {
   return rf::capture_graph(s, "rf_dit", step, &g->exec, &g->kernels);
 }
 
-// rf_dit_denoise, and with uncond_latents != nullptr rf_dit_denoise_image_guidance (arguments checked by the caller)
-static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
-                        const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
-                        float guidance_scale, const void* cond_latents, const bf16* uncond_latents,
-                        float image_guidance_scale, void* stream) {
-  const bool guided = uncond_latents != nullptr;
-  // The loop runs on the handle's side stream, so the step can be captured whatever stream the caller passes
-  cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  cudaStream_t s = nullptr;
-  RF_TRY(h->side.enter(caller, &s));
-  const int C = h->cfg.in_channels;
+// The schedule of an n_steps loop on stream s: the schedule arrays and step tables grow with n_steps (the captured
+// step references them, so growing drops it), then timesteps, sigmas, guidance and (guided) s are uploaded.
+static int stage_schedule(rf_dit* h, const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                          float guidance_scale, bool guided, float image_guidance_scale, cudaStream_t s) {
   if (n_steps > h->s_cap_steps) {
     RF_TRY(h->geo_mem.alloc(&h->s_tsteps, n_steps));
     RF_TRY(h->geo_mem.alloc(&h->s_sigmas, n_steps + 1));
@@ -1218,6 +1229,22 @@ static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const v
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_guid, &gb, 2, cudaMemcpyHostToDevice, s));
   if (guided)
     RF_CHECK_CUDA(cudaMemcpyAsync(h->s_igs, &image_guidance_scale, 4, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// rf_dit_denoise, and with uncond_latents != nullptr rf_dit_denoise_image_guidance (arguments checked by the caller)
+static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
+                        const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                        float guidance_scale, const void* cond_latents, const bf16* uncond_latents,
+                        float image_guidance_scale, void* stream) {
+  const bool guided = uncond_latents != nullptr;
+  // The loop runs on the handle's side stream, so the step can be captured whatever stream the caller passes
+  cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  cudaStream_t s = nullptr;
+  RF_TRY(h->side.enter(caller, &s));
+  h->sess = false;  // this loop rewrites the step's staging and tables
+  const int C = h->cfg.in_channels;
+  RF_TRY(stage_schedule(h, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, guided, image_guidance_scale, s));
   StepGraph* g = guided ? &h->graph_ig : &h->graph;
   const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
 
@@ -1299,6 +1326,134 @@ int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* tx
   }
   return denoise_loop(h, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale,
                       cond_latents, static_cast<const bf16*>(uncond_latents), image_guidance_scale, stream);
+}
+
+int rf_dit_denoise_begin(rf_dit* h, const void* pooled, const uint16_t* timesteps_bf16_host, const float* sigmas_host,
+                         int n_steps, float guidance_scale, const void* cond_latents, float image_guidance_scale,
+                         void* stream) {
+  int rc = check_ready(h, "rf_dit_denoise_begin", static_cast<cudaStream_t>(stream));
+  if (rc) return rc;
+  h->sess = false;
+  if (!pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 || (h->n_cond > 0 && !cond_latents)) {
+    rf::set_error("rf_dit_denoise_begin: bad argument");
+    return -1;
+  }
+  const bool guided = image_guidance_scale != 1.0f;
+  if (guided && (h->n_cond <= 0 || !h->cfg.guidance_embeds)) {
+    rf::set_error("rf_dit_denoise_begin: image_guidance_scale != 1 needs a condition stream (n_cond > 0) and "
+                  "guidance_embeds");
+    return -1;
+  }
+  if (!std::isfinite(image_guidance_scale)) {
+    rf::set_error("rf_dit_denoise_begin: image_guidance_scale must be finite");
+    return -1;
+  }
+  cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  cudaStream_t s = nullptr;
+  RF_TRY(h->side.enter(caller, &s));
+  const int C = h->cfg.in_channels, B = h->batch;
+  RF_TRY(stage_schedule(h, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, guided, image_guidance_scale, s));
+  rf::DeviceAllocs& gm = h->geo_mem;
+  const int64_t rows = static_cast<int64_t>(B) * n_steps;
+  if (rows > h->sess_rows) {
+    gm.release(h->sess_mod);
+    RF_TRY(gm.alloc(&h->sess_mod, static_cast<size_t>(rows) * h->n_mod));
+    h->sess_rows = rows;
+  }
+  if (guided && rows > h->sess_rows_u) {
+    gm.release(h->sess_mod_u);
+    RF_TRY(gm.alloc(&h->sess_mod_u, static_cast<size_t>(rows) * h->n_mod));
+    h->sess_rows_u = rows;
+  }
+  if (n_steps > h->sess_idx_n) {
+    gm.release(h->sess_idx);
+    RF_TRY(gm.alloc(&h->sess_idx, n_steps));
+    std::vector<int> idx(n_steps);
+    for (int i = 0; i < n_steps; ++i) idx[i] = i;
+    RF_CHECK_CUDA(cudaMemcpyAsync(h->sess_idx, idx.data(), static_cast<size_t>(n_steps) * 4, cudaMemcpyHostToDevice, s));
+    h->sess_idx_n = n_steps;
+  }
+  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
+  if (h->n_cond > 0) {
+    if (!h->sess_modc) RF_TRY(gm.alloc(&h->sess_modc, static_cast<size_t>(B) * h->n_mod));
+    if (!h->sess_cond) RF_TRY(gm.alloc(&h->sess_cond, B * cond_elems));
+    RF_CHECK_CUDA(cudaMemcpyAsync(h->sess_cond, cond_latents, B * cond_elems * 2, cudaMemcpyDeviceToDevice, s));
+  }
+  // the tables of every sample, by the same temb_mod calls as the whole loop: bit-identical rows
+  for (int b = 0; b < B; ++b) {
+    const bf16* pool_b = static_cast<const bf16*>(pooled) + static_cast<int64_t>(b) * h->cfg.pooled_projection_dim;
+    const int64_t row0 = static_cast<int64_t>(b) * n_steps * h->n_mod;
+    if (h->n_cond > 0) RF_TRY(compute_cond_mod(h, pool_b, s, h->sess_modc + static_cast<int64_t>(b) * h->n_mod));
+    RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, pool_b, (h->flags & 1) != 0, true, h->sess_mod + row0,
+                    h->s_temb_ws, s));
+    if (guided)
+      RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_zero_one + 1, pool_b, (h->flags & 1) != 0, true,
+                      h->sess_mod_u + row0, h->s_temb_ws, s));
+  }
+  StepGraph* g = guided ? &h->graph_ig : &h->graph;
+  if (g->exec && g->call_scale != h->call_scale) drop_graph(h);
+  if (!g->exec) RF_TRY(capture_step(h, guided, g, s));
+  h->sess = true;
+  h->sess_guided = guided;
+  h->sess_steps = n_steps;
+  return h->side.leave(caller);
+}
+
+int rf_dit_denoise_step(rf_dit* h, int i, void* latents_inout, const void* txt, const void* uncond_latents_i,
+                        void* stream) {
+  if (!h) {
+    rf::set_error("rf_dit_denoise_step: null handle");
+    return -1;
+  }
+  if (!h->sess) {
+    rf::set_error("rf_dit_denoise_step: no open session: call rf_dit_denoise_begin (rf_dit_prepare, LoRA and "
+                  "weight changes, the LoRA call scale and a whole-loop denoise close it)");
+    return -1;
+  }
+  if (i < 0 || i >= h->sess_steps) {
+    rf::set_error("rf_dit_denoise_step: step " + std::to_string(i) + " outside [0, " +
+                  std::to_string(h->sess_steps) + ")");
+    return -1;
+  }
+  if (!latents_inout || !txt || (uncond_latents_i != nullptr) != h->sess_guided) {
+    rf::set_error(h->sess_guided ? "rf_dit_denoise_step: bad argument (an image-guided session needs uncond_latents_i)"
+                                 : "rf_dit_denoise_step: bad argument (uncond_latents_i is for image-guided sessions)");
+    return -1;
+  }
+  cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  cudaStream_t s = nullptr;
+  RF_TRY(h->side.enter(caller, &s));
+  const int C = h->cfg.in_channels;
+  const size_t lat_bytes = static_cast<size_t>(h->n_img) * C * 2;
+  const size_t txt_elems = static_cast<size_t>(h->n_txt) * h->cfg.joint_attention_dim;
+  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
+  const size_t mod_bytes = static_cast<size_t>(h->n_mod) * 2;
+  const StepGraph* g = h->sess_guided ? &h->graph_ig : &h->graph;
+  auto d2d = [&](void* dst, const void* src, size_t bytes) {
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
+  };
+  for (int b = 0; b < h->batch; ++b) {
+    bf16* lat_b = static_cast<bf16*>(latents_inout) + static_cast<int64_t>(b) * h->n_img * C;
+    const int64_t row = static_cast<int64_t>(b) * h->sess_steps + i;
+    RF_CHECK_CUDA(d2d(h->s_lat, lat_b, lat_bytes));
+    RF_CHECK_CUDA(d2d(h->s_txt, static_cast<const bf16*>(txt) + b * txt_elems, txt_elems * 2));
+    // the captured step selects row *s_step of s_mod_all: put sample b's row i there
+    RF_CHECK_CUDA(d2d(h->s_mod_all + static_cast<int64_t>(i) * h->n_mod, h->sess_mod + row * h->n_mod, mod_bytes));
+    if (h->n_cond > 0) {
+      RF_CHECK_CUDA(d2d(h->s_cond, h->sess_cond + b * cond_elems, cond_elems * 2));
+      RF_CHECK_CUDA(d2d(h->MODC, h->sess_modc + static_cast<int64_t>(b) * h->n_mod, mod_bytes));
+    }
+    if (h->sess_guided) {
+      RF_CHECK_CUDA(d2d(h->s_mod_all_u + static_cast<int64_t>(i) * h->n_mod, h->sess_mod_u + row * h->n_mod,
+                        mod_bytes));
+      RF_CHECK_CUDA(d2d(h->s_ucond, static_cast<const bf16*>(uncond_latents_i) + b * cond_elems, cond_elems * 2));
+    }
+    RF_CHECK_CUDA(d2d(h->s_step, h->sess_idx + i, sizeof(int)));
+    RF_CHECK_CUDA(cudaGraphLaunch(g->exec, s));
+    rf::count_launch(static_cast<int>(g->kernels));
+    RF_CHECK_CUDA(d2d(lat_b, h->s_lat, lat_bytes));
+  }
+  return h->side.leave(caller);
 }
 
 }  // extern "C"

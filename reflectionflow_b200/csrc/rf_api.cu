@@ -23,6 +23,7 @@ const char* get_error() { return g_err.c_str(); }
 static std::atomic<int64_t> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int64_t launch_count() { return g_launches.load(std::memory_order_relaxed); }
+static std::atomic<int64_t> g_captures{0};
 
 int require_device(const char* who) {
   int ndev = 0;
@@ -108,6 +109,7 @@ void SideStream::destroy() {
 int capture_graph(cudaStream_t s, const char* who, const std::function<int()>& body, cudaGraphExec_t* exec,
                   int64_t* launches) {
   RF_CHECK_CUDA(cudaStreamSynchronize(s));
+  g_captures.fetch_add(1, std::memory_order_relaxed);
   const int64_t before = launch_count();
   RF_CHECK_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
   int rc = body();
@@ -385,6 +387,7 @@ int rf_dbg_vae_sample_pack(const void* mom, int C, const void* eps, void* packed
 const char* rf_last_error(void) { return rf::get_error(); }
 int rf_abi_version(void) { return RF_B200_ABI_VERSION; }
 int64_t rf_launch_count(void) { return rf::launch_count(); }
+int64_t rf_graph_capture_count(void) { return rf::g_captures.load(std::memory_order_relaxed); }
 
 int rf_profile_start(void) {
   for (auto& r : rf::g_prof) {

@@ -140,6 +140,7 @@ class Condition:
 class B200FluxPipeline:
     vae_scale_factor = 8
     default_sample_size = 128
+    _callback_tensor_inputs = ["latents", "prompt_embeds"]
 
     def __init__(self, transformer: B200FluxTransformer2DModel,
                  text_encoder_hook: Optional[Callable] = None, vae=None):
@@ -278,6 +279,10 @@ class B200FluxPipeline:
                              "passed.")
         if max_sequence_length is not None and max_sequence_length > 512:
             raise ValueError(f"`max_sequence_length` cannot be greater than 512 but is {max_sequence_length}")
+        if callback_on_step_end_tensor_inputs is not None and not all(
+                k in self._callback_tensor_inputs for k in callback_on_step_end_tensor_inputs):
+            raise ValueError(f"`callback_on_step_end_tensor_inputs` has to be in {self._callback_tensor_inputs}, but "
+                             f"found {[k for k in callback_on_step_end_tensor_inputs if k not in self._callback_tensor_inputs]}")
 
     def encode_prompt(self, prompt=None, prompt_2=None, device=None, num_images_per_prompt: int = 1,
                       prompt_embeds=None, pooled_prompt_embeds=None, max_sequence_length: int = 512,
@@ -366,7 +371,7 @@ class B200FluxPipeline:
     def _denoise(self, latents, prompt_embeds, pooled, text_ids, image_ids, num_inference_steps,
                  guidance_scale, timesteps=None, condition_latents=None, condition_ids=None,
                  model_config=None, condition_scale: float = 1.0, image_guidance_scale: float = 1.0,
-                 uncond_latents=None):
+                 uncond_latents=None, callback_on_step_end=None, callback_on_step_end_tensor_inputs=("latents",)):
         if timesteps is not None:
             raise NotImplementedError("custom `timesteps` are not supported (the reference passes sigmas)")
         sigmas = np.linspace(1.0, 1 / num_inference_steps, num_inference_steps)
@@ -378,12 +383,30 @@ class B200FluxPipeline:
         self._num_timesteps = len(ts)
         # generate.py:222,240: t -> latents dtype (bf16), then / 1000 in bf16
         t_in = ts.to(self.dtype) / 1000
+        hook = None
+        if callback_on_step_end is not None:
+            hook = self._step_hook(callback_on_step_end, callback_on_step_end_tensor_inputs, ts)
         return self.transformer.denoise(latents, prompt_embeds, pooled, t_in, self.scheduler.sigmas,
                                         guidance_scale, image_ids, text_ids, condition_latents,
                                         condition_ids, model_config, condition_scale,
                                         **({} if image_guidance_scale == 1.0 else dict(
                                             image_guidance_scale=image_guidance_scale,
-                                            uncond_condition_latents=uncond_latents)))
+                                            uncond_condition_latents=uncond_latents)),
+                                        **({} if hook is None else dict(step_hook=hook)))
+
+    def _step_hook(self, callback, tensor_inputs, timesteps):
+        """generate.py:283-290 as a step hook of `transformer.denoise`: after step i, `callback(self, i, t,
+        callback_kwargs)` with t = scheduler.timesteps[i] (0-d fp32 on the device) and the tensors named by
+        `tensor_inputs`; its "latents" / "prompt_embeds" feed the next step, or are the result of the call (other keys
+        are ignored, as the reference's `pop`).  Once the callback sets `self._interrupt`, no further step runs
+        (generate.py:218-219), and the latents it returned in that step are the result."""
+        ts = timesteps.to(self.device)
+
+        def hook(i, latents, prompt_embeds):
+            tensors = {"latents": latents, "prompt_embeds": prompt_embeds}
+            out = callback(self, i, ts[i], {k: tensors[k] for k in tensor_inputs})
+            return out.pop("latents", latents), out.pop("prompt_embeds", prompt_embeds), self.interrupt
+        return hook
 
     def _finish(self, latents, height, width, output_type, return_dict):
         if output_type == "latent":
@@ -425,8 +448,6 @@ class B200FluxPipeline:
                           pooled_prompt_embeds=pooled_prompt_embeds,
                           callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs,
                           max_sequence_length=max_sequence_length)
-        if callback_on_step_end is not None:
-            raise NotImplementedError("per-step callbacks would break the graph-captured loop")
         self._guidance_scale = guidance_scale
         self._joint_attention_kwargs = joint_attention_kwargs
         self._interrupt = False
@@ -446,7 +467,9 @@ class B200FluxPipeline:
             batch_size * num_images_per_prompt, num_channels_latents, height, width,
             prompt_embeds.dtype, device, generator, latents)
         latents = self._denoise(latents, prompt_embeds, pooled_prompt_embeds, text_ids,
-                                latent_image_ids, num_inference_steps, guidance_scale, timesteps)
+                                latent_image_ids, num_inference_steps, guidance_scale, timesteps,
+                                callback_on_step_end=callback_on_step_end,
+                                callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs)
         return self._finish(latents, height, width, output_type, return_dict)
 
 
@@ -507,13 +530,11 @@ def generate(pipeline: B200FluxPipeline, conditions: List[Condition] = None, con
     prompt_embeds = params.get("prompt_embeds")
     pooled_prompt_embeds = params.get("pooled_prompt_embeds")
     max_sequence_length = params.get("max_sequence_length", 512)
+    callback_on_step_end_tensor_inputs = params.get("callback_on_step_end_tensor_inputs", ["latents"])
     self.check_inputs(prompt, prompt_2, height, width, prompt_embeds=prompt_embeds,
                       pooled_prompt_embeds=pooled_prompt_embeds,
-                      callback_on_step_end_tensor_inputs=params.get(
-                          "callback_on_step_end_tensor_inputs", ["latents"]),
+                      callback_on_step_end_tensor_inputs=callback_on_step_end_tensor_inputs,
                       max_sequence_length=max_sequence_length)
-    if params.get("callback_on_step_end") is not None:
-        raise NotImplementedError("per-step callbacks would break the graph-captured loop")
     self._guidance_scale = guidance_scale
     self._joint_attention_kwargs = params.get("joint_attention_kwargs")
     self._interrupt = False
@@ -551,6 +572,7 @@ def generate(pipeline: B200FluxPipeline, conditions: List[Condition] = None, con
     with lora_scale(self.transformer, self._joint_attention_kwargs):
         latents = self._denoise(latents, prompt_embeds, pooled_prompt_embeds, text_ids, latent_image_ids,
                                 num_inference_steps, guidance_scale, params.get("timesteps"), cond_lat,
-                                cond_ids, model_config, condition_scale, image_guidance_scale, unc_lat)
+                                cond_ids, model_config, condition_scale, image_guidance_scale, unc_lat,
+                                params.get("callback_on_step_end"), callback_on_step_end_tensor_inputs)
     return self._finish(latents, height, width, params.get("output_type", "pil"),
                         params.get("return_dict", True))

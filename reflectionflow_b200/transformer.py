@@ -325,13 +325,16 @@ class B200FluxTransformer2DModel:
                 sigmas_f32: torch.Tensor, guidance_scale: float, img_ids, txt_ids,
                 condition_latents=None, condition_ids=None, model_config=None,
                 condition_scale: float = 1.0, image_guidance_scale: float = 1.0,
-                uncond_condition_latents=None) -> torch.Tensor:
+                uncond_condition_latents=None, step_hook=None) -> torch.Tensor:
         """Whole denoise loop on the device (rf_dit_denoise): one CUDA graph per step, replayed.
 
         `image_guidance_scale` s != 1: image classifier-free guidance over the condition stream (generate.py:250-272,
         rf_dit_denoise_image_guidance).  Every step adds a forward with the condition latents U_i of
         `uncond_condition_latents` [B, n_steps, n_cond, 64] and guidance 1, and steps on u + s * (c - u).  Without
-        them U_i = condition_latents for every step.  s == 1 is the plain loop and ignores them."""
+        them U_i = condition_latents for every step.  s == 1 is the plain loop and ignores them.
+
+        `step_hook(i, latents, prompt_embeds)` runs the loop step by step (rf_dit_denoise_begin / _step): see
+        `run_steps`.  Without a hook the loop is one rf_dit_denoise call."""
         B = latents.shape[0]
         ts = timesteps_bf16.detach().to("cpu", torch.bfloat16).contiguous().view(torch.int16)
         sg = sigmas_f32.detach().to("cpu", torch.float32).contiguous()
@@ -361,6 +364,10 @@ class B200FluxTransformer2DModel:
         txt = _bf16c(prompt_embeds, dev)
         pool = _bf16c(pooled, dev)
         cond = _bf16c(condition_latents, dev) if condition_latents is not None else None
+        if step_hook is not None:
+            unc = _bf16c(uncond_condition_latents, dev) if guided else None
+            return self._denoise_steps(lat, txt, pool, ts, sg, guidance_scale, cond, image_guidance_scale if guided
+                                       else 1.0, unc, step_hook)
         with torch.cuda.device(dev):
             if guided:
                 unc = _bf16c(uncond_condition_latents, dev)
@@ -376,6 +383,49 @@ class B200FluxTransformer2DModel:
                                                  L.cur_stream()), "rf_dit_denoise")
             torch.cuda.current_stream().synchronize()  # ts/sg host buffers must outlive the copies
         return lat
+
+    def _denoise_steps(self, lat, txt, pool, ts, sg, guidance_scale, cond, image_guidance_scale, unc, step_hook):
+        """The loop of `denoise` with a step hook: one session, then one rf_dit_denoise_step per executed step."""
+        n = ts.numel()
+        with torch.cuda.device(self.device):
+            L.check(self._lib.rf_dit_denoise_begin(
+                self._h, L.ptr(pool), ctypes.c_void_p(ts.data_ptr()), ctypes.c_void_p(sg.data_ptr()), n,
+                ctypes.c_float(guidance_scale), L.ptr(cond), ctypes.c_float(image_guidance_scale), L.cur_stream()),
+                "rf_dit_denoise_begin")
+            torch.cuda.current_stream().synchronize()  # ts/sg host buffers must outlive the copies
+
+            def step(i, lat, txt):
+                u_i = None if unc is None else unc[:, i].contiguous()
+                L.check(self._lib.rf_dit_denoise_step(self._h, i, L.ptr(lat), L.ptr(txt), L.ptr(u_i),
+                                                      L.cur_stream()), "rf_dit_denoise_step")
+            return run_steps(n, step, step_hook, lat, txt)
+
+
+def run_steps(n: int, step, step_hook, lat: torch.Tensor, txt: torch.Tensor) -> torch.Tensor:
+    """The step-wise loop of `denoise` (generate.py:217-290).  For i < n: `step(i, lat, txt)` advances a new copy of
+    the latents in place (a new tensor per step, as the reference's scheduler.step returns one: a callback may keep
+    it), then `step_hook(i, lat, txt)` returns (latents, prompt_embeds, stop).  The returned tensors feed the next
+    step, or are the result when `stop` is set or i is the last step, as the reference pops the callback's outputs
+    before its interrupt check.  They must keep the shapes and be bf16, else ValueError."""
+    for i in range(n):
+        lat = lat.clone()
+        step(i, lat, txt)
+        new_lat, new_txt, stop = step_hook(i, lat, txt)
+        # the next step reads these through raw pointers
+        lat, txt = step_input(new_lat, lat, "latents"), step_input(new_txt, txt, "prompt_embeds")
+        if stop:
+            break
+    return lat
+
+
+def step_input(t, ref: torch.Tensor, name: str) -> torch.Tensor:
+    """A tensor a step callback hands to the next denoise step, on `ref`'s device and contiguous.  Its shape and dtype
+    must be `ref`'s: the step reads that many bf16 rows."""
+    if not torch.is_tensor(t) or t.shape != ref.shape or t.dtype != torch.bfloat16:
+        got = f"{tuple(t.shape)} {t.dtype}" if torch.is_tensor(t) else type(t).__name__
+        raise ValueError(f"`{name}` returned by callback_on_step_end must be a bf16 tensor of shape "
+                         f"{tuple(ref.shape)}, got {got}")
+    return t.detach().to(ref.device).contiguous()
 
 
 @contextmanager
