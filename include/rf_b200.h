@@ -214,7 +214,8 @@ int rf_dit_forward(rf_dit* h, const void* latents, const void* txt, const void* 
 /* The whole denoise loop of generate() / FluxPipeline.__call__ (generate.py:217-276):
  * n_steps x (forward + Euler step), latents updated in place.  timesteps: HOST bf16 [n_steps]
  * (the bf16(t)/1000 values the reference feeds), sigmas: HOST fp32 [n_steps+1].  The step body is
- * captured once into a CUDA graph and replayed. */
+ * captured once into a CUDA graph and replayed.  The call is rf_dit_denoise_begin, then rf_dit_denoise_step
+ * 0 .. n_steps-1, and leaves no session open. */
 int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
                    const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
                    float guidance_scale, const void* cond_latents, void* stream);
@@ -248,10 +249,10 @@ int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* tx
  *
  * rf_dit_denoise_step runs step i for every sample, in place on latents_inout [B, n_img, 64], with txt
  * [B, n_txt, 4096] as the text input; an image-guided session takes that step's uncond condition latents
- * uncond_latents_i [B, n_cond, 64], an unguided one NULL.  Per sample it copies the latents, text, condition and
- * U_i into the captured step's staging, copies the sample's table rows into the rows the step selects and the step
- * index from device memory (no host-to-device copy), replays the graph and copies the latents back: no host
- * synchronisation, no capture.  Steps may run in any order and repeat; running 0 .. n_steps-1 once each on
+ * uncond_latents_i [B, n_cond, 64], an unguided one NULL.  Per sample it copies the latents, text, condition, its
+ * cond_temb vectors and U_i into the captured step's staging, sets the row index (the sample's row of each table)
+ * and the step index from device memory (no host-to-device copy), replays the graph and copies the latents back:
+ * no host synchronisation, no capture.  Steps may run in any order and repeat; running 0 .. n_steps-1 once each on
  * unchanged inputs gives rf_dit_denoise's bytes.
  *
  * rf_dit_prepare, rf_dit_load_weight, rf_dit_set_lora, rf_dit_clear_lora, rf_dit_set_lora_scale, rf_dit_denoise,

@@ -135,33 +135,30 @@ struct rf_dit {
   bf16 *LT = nullptr, *LL = nullptr;  // LoRA temporaries: T [lora_rows, 4 lora_pad], L [lora_rows, 4D]
   int lora_rows = 0;
   bf16* emb_ws = nullptr;             // temb_mod workspace of one vector (eager step, cond_temb)
-  // ---- staging for the graph-captured denoise loop
-  bf16 *s_lat = nullptr, *s_txt = nullptr, *s_pooled = nullptr, *s_cond = nullptr, *s_v = nullptr;
+  // ---- the denoise loop (rf_dit_denoise, rf_dit_denoise_image_guidance, rf_dit_denoise_begin / _step)
+  // Staging of the captured step, one sample: before each replay the loop copies a sample's inputs here, and the
+  // step's sigma index into s_step and its table row into s_row.
+  bf16 *s_lat = nullptr, *s_txt = nullptr, *s_cond = nullptr, *s_v = nullptr;
   bf16 *s_tsteps = nullptr, *s_guid = nullptr, *s_zero_one = nullptr;
   float* s_sigmas = nullptr;
-  int* s_step = nullptr;
-  // every step's adaLN modulation vectors, computed BEFORE the loop (all timesteps are known up
-  // front): MOD_ALL [n_steps, n_mod]; the captured step only selects its row
-  bf16 *s_mod_all = nullptr, *s_temb_ws = nullptr;
-  int s_cap_steps = 0;
-  // image guidance (rf_dit_denoise_image_guidance): the uncond branch's table MOD_ALL at guidance bf16(1) (same
-  // layout, s_cap_steps_u rows), its condition input U_i and noise prediction, and the scale s (device fp32)
-  bf16 *s_mod_all_u = nullptr, *s_ucond = nullptr, *s_vu = nullptr;
+  int *s_step = nullptr, *s_row = nullptr;
+  // image guidance: the uncond branch's condition input U_i and noise prediction, and the scale s (device fp32)
+  bf16 *s_ucond = nullptr, *s_vu = nullptr;
   float* s_igs = nullptr;
-  int s_cap_steps_u = 0;
-  StepGraph graph, graph_ig;  // the captured step of rf_dit_denoise / of the guided loop
+  // The tables of the open loop, built when it opens (all timesteps are known up front): every sample's adaLN
+  // modulation vectors of every step, tab [B n_steps, n_mod] (row b n_steps + i), with image guidance also the
+  // uncond branch's tab_u at guidance bf16(1); every sample's cond_temb vectors tab_c [B, n_mod] and condition
+  // latents loop_cond [B, n_cond, C]; idx = 0, 1, ..., B tab_steps - 1, the source of s_step and s_row.
+  // s_tsteps, s_sigmas, tab, tab_u, temb_ws and idx hold tab_steps steps and grow with n_steps.
+  bf16 *tab = nullptr, *tab_u = nullptr, *tab_c = nullptr, *loop_cond = nullptr, *temb_ws = nullptr;
+  int* idx = nullptr;
+  int tab_steps = 0;
+  StepGraph graph, graph_ig;  // the captured step of the plain / of the image-guided loop
   rf::SideStream side;        // the denoise loop's stream
-  // step-wise session (rf_dit_denoise_begin / rf_dit_denoise_step): every sample's tables, built once at begin.
-  // Before each replay of the captured step, sample b's row i is copied into the row the step selects
-  // (s_mod_all[i], s_mod_all_u[i]) and its cond_temb table into MODC.  Everything that drops the captured step or
-  // changes what the tables were built from closes the session (sess = false).
+  // The open loop's step count and kind.  sess: rf_dit_denoise_begin opened it; everything that drops the captured
+  // step or changes what the tables were built from closes it.
   bool sess = false, sess_guided = false;
   int sess_steps = 0;
-  int64_t sess_rows = 0, sess_rows_u = 0;  // rows of sess_mod / sess_mod_u (B x n_steps)
-  bf16 *sess_mod = nullptr, *sess_mod_u = nullptr;  // [B, n_steps, n_mod]
-  bf16 *sess_modc = nullptr, *sess_cond = nullptr;  // [B, n_mod] cond_temb tables, [B, n_cond, C] condition latents
-  int* sess_idx = nullptr;                          // 0, 1, ..., sess_idx_n - 1: the step index copied into s_step
-  int sess_idx_n = 0;
 };
 
 namespace {
@@ -586,9 +583,10 @@ int project(rf_dit* h, int epi, int N, int K, Proj& pr, cudaStream_t s, const bf
   return rf::gemm_launch(epi, N, K, pr.n, pr.g, s);
 }
 
-// The body of one DiT forward for one sample.  All pointers are device pointers.
+// The body of one DiT forward for one sample.  All pointers are device pointers.  mod_all != nullptr: the step's
+// modulation vectors are row *row of that table (pooled, tstep and guid are not read).
 int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16* pooled,
-                    const bf16* tstep, const int* step_idx, const bf16* guid, const bf16* cond_lat,
+                    const bf16* tstep, const int* row, const bf16* guid, const bf16* cond_lat,
                     bf16* out, cudaStream_t s, const bf16* mod_all = nullptr) {
   const int D = h->D, D3 = 3 * D, D4 = 4 * D, D5 = 5 * D, C = h->cfg.in_channels, lpad = h->lora_pad;
   const bool use_cond = h->n_cond > 0;
@@ -616,7 +614,7 @@ int enqueue_forward(rf_dit* h, const bf16* latents, const bf16* txt, const bf16*
 
   // ---- temb and every modulation vector of the step (transformer.py:95-107 + all adaLN linears)
   if (mod_all != nullptr) {  // denoise loop: this step's row of the precomputed table
-    RF_TRY(rf::select_row_launch(mod_all, h->n_mod, step_idx, h->MOD, s));
+    RF_TRY(rf::select_row_launch(mod_all, h->n_mod, row, h->MOD, s));
   } else {
     RF_TRY(temb_mod(h, 1, tstep, guid, pooled, (h->flags & 1) != 0, true, h->MOD, h->emb_ws, s));
   }
@@ -762,15 +760,10 @@ void free_geometry(rf_dit* h) {
   h->geo_mem.release_all();
   h->prepared = false;
   h->lora_rows = 0;
-  h->s_cap_steps = 0;
-  h->s_tsteps = nullptr;
+  h->tab_steps = 0;
+  h->s_tsteps = h->tab = h->tab_u = h->temb_ws = nullptr;
   h->s_sigmas = nullptr;
-  h->s_cap_steps_u = 0;
-  h->s_mod_all_u = nullptr;
-  h->sess_rows = h->sess_rows_u = 0;
-  h->sess_mod = h->sess_mod_u = h->sess_modc = h->sess_cond = nullptr;
-  h->sess_idx = nullptr;
-  h->sess_idx_n = 0;
+  h->idx = nullptr;
 }
 
 }  // namespace
@@ -1079,24 +1072,22 @@ int rf_dit_prepare(rf_dit* h, int batch, int n_txt, int n_img, int n_cond, const
     RF_TRY(alloc_lora_ws(h, lora_rows));
     RF_TRY(g.alloc(&h->emb_ws, temb_ws_elems(h, 1)));
     const int C = h->cfg.in_channels;
-    RF_TRY(g.alloc(&h->s_lat, static_cast<size_t>(batch) * n_img * C));
-    RF_TRY(g.alloc(&h->s_v, static_cast<size_t>(batch) * n_img * C));
-    RF_TRY(g.alloc(&h->s_txt, static_cast<size_t>(batch) * n_txt * h->cfg.joint_attention_dim));
-    RF_TRY(g.alloc(&h->s_pooled, static_cast<size_t>(batch) * h->cfg.pooled_projection_dim));
-    RF_TRY(g.alloc(&h->s_cond, batch * nc * C));
+    RF_TRY(g.alloc(&h->s_lat, static_cast<size_t>(n_img) * C));
+    RF_TRY(g.alloc(&h->s_v, static_cast<size_t>(n_img) * C));
+    RF_TRY(g.alloc(&h->s_txt, static_cast<size_t>(n_txt) * h->cfg.joint_attention_dim));
+    RF_TRY(g.alloc(&h->s_cond, nc * C));
     RF_TRY(g.alloc(&h->s_guid, static_cast<size_t>(batch) + 8));
     RF_TRY(g.alloc(&h->s_zero_one, 8));
     RF_TRY(g.alloc(&h->s_step, 4));
-    if (n_cond > 0) {  // image guidance needs a condition stream
+    RF_TRY(g.alloc(&h->s_row, 4));
+    if (n_cond > 0) {
+      RF_TRY(g.alloc(&h->tab_c, static_cast<size_t>(batch) * h->n_mod));
+      RF_TRY(g.alloc(&h->loop_cond, static_cast<size_t>(batch) * n_cond * C));
+      // image guidance needs a condition stream
       RF_TRY(g.alloc(&h->s_ucond, static_cast<size_t>(n_cond) * C));
       RF_TRY(g.alloc(&h->s_vu, static_cast<size_t>(n_img) * C));
       RF_TRY(g.alloc(&h->s_igs, 4));
     }
-    h->s_cap_steps = 0;
-    h->s_tsteps = nullptr;
-    h->s_sigmas = nullptr;
-    h->s_cap_steps_u = 0;
-    h->s_mod_all_u = nullptr;
     const uint16_t zo[2] = {0x0000, 0x3F80};  // bf16 0.0, 1.0
     RF_CHECK_CUDA(cudaMemcpy(h->s_zero_one, zo, sizeof(zo), cudaMemcpyHostToDevice));
   }
@@ -1183,44 +1174,72 @@ int rf_dit_forward(rf_dit* h, const void* latents, const void* txt, const void* 
   return 0;
 }
 
-// Capture one step of the denoise loop into g: forward -> Euler update -> step counter, or with image guidance
-// forward (cond) -> forward (uncond: its own modulation table, condition input U_i) -> guidance + Euler -> counter.
+// Capture one step of the denoise loop into g: forward -> Euler update, or with image guidance forward (cond) ->
+// forward (uncond: its own modulation table, condition input U_i) -> guidance + Euler.  Both forwards read the table
+// row at s_row, the update reads the sigmas at s_step.
 static int capture_step(rf_dit* h, bool guided, StepGraph* g, cudaStream_t s) {
   const int C = h->cfg.in_channels;
   g->call_scale = h->call_scale;
   auto step = [&]() {
-    RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_guid,
-                           h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s, h->s_mod_all));
-    if (guided) {
-      RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, h->s_pooled, h->s_tsteps, h->s_step, h->s_zero_one + 1,
-                             h->s_ucond, h->s_vu, s, h->s_mod_all_u));
-      RF_TRY(rf::image_guidance_step_launch(h->s_lat, h->s_v, h->s_vu, h->s_igs, h->s_sigmas, h->s_step,
-                                            h->n_img * C, s));
-    } else {
-      RF_TRY(rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s));
-    }
-    return rf::advance_step_launch(h->s_step, s);
+    RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, nullptr, nullptr, h->s_row, nullptr,
+                           h->n_cond > 0 ? h->s_cond : nullptr, h->s_v, s, h->tab));
+    if (!guided) return rf::euler_step_launch(h->s_lat, h->s_v, h->s_sigmas, h->s_step, h->n_img * C, s);
+    RF_TRY(enqueue_forward(h, h->s_lat, h->s_txt, nullptr, nullptr, h->s_row, nullptr, h->s_ucond, h->s_vu, s,
+                           h->tab_u));
+    return rf::image_guidance_step_launch(h->s_lat, h->s_v, h->s_vu, h->s_igs, h->s_sigmas, h->s_step, h->n_img * C,
+                                          s);
   };
   return rf::capture_graph(s, "rf_dit", step, &g->exec, &g->kernels);
 }
 
-// The schedule of an n_steps loop on stream s: the schedule arrays and step tables grow with n_steps (the captured
-// step references them, so growing drops it), then timesteps, sigmas, guidance and (guided) s are uploaded.
-static int stage_schedule(rf_dit* h, const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
-                          float guidance_scale, bool guided, float image_guidance_scale, cudaStream_t s) {
-  if (n_steps > h->s_cap_steps) {
-    RF_TRY(h->geo_mem.alloc(&h->s_tsteps, n_steps));
-    RF_TRY(h->geo_mem.alloc(&h->s_sigmas, n_steps + 1));
-    RF_TRY(h->geo_mem.alloc(&h->s_mod_all, static_cast<size_t>(n_steps) * h->n_mod));
-    RF_TRY(h->geo_mem.alloc(&h->s_temb_ws, temb_ws_elems(h, n_steps)));
-    h->s_cap_steps = n_steps;
-    drop_graph(h);  // graph referenced the old arrays
+// The checks of the three loop entry points; who names the entry point in the messages.  inputs_ok: the whole
+// loop's own inputs are there (begin has none).  On a ready handle the call closes the step session first.
+static int check_loop(rf_dit* h, const char* who, cudaStream_t s, bool inputs_ok, const void* pooled,
+                      const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
+                      const void* cond_latents, bool guided, float image_guidance_scale) {
+  RF_TRY(check_ready(h, who, s));
+  h->sess = false;
+  if (!inputs_ok || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 ||
+      (h->n_cond > 0 && !cond_latents)) {
+    rf::set_error(std::string(who) + ": bad argument");
+    return -1;
   }
-  if (guided && n_steps > h->s_cap_steps_u) {
-    RF_TRY(h->geo_mem.alloc(&h->s_mod_all_u, static_cast<size_t>(n_steps) * h->n_mod));
-    h->s_cap_steps_u = n_steps;
+  if (guided && (h->n_cond <= 0 || !h->cfg.guidance_embeds)) {
+    rf::set_error(std::string(who) + ": image guidance needs a condition stream (n_cond > 0) and guidance_embeds");
+    return -1;
+  }
+  if (!std::isfinite(image_guidance_scale)) {
+    rf::set_error(std::string(who) + ": image_guidance_scale must be finite");
+    return -1;
+  }
+  return 0;
+}
+
+// Open a loop of n_steps on stream s: upload the schedule, build every sample's tables (by the temb_mod calls of the
+// eager forward: bit-identical rows), stage the condition latents, and capture the step unless the current one was
+// built for this call scale.  Growing the tables drops the captured step, which reads them.
+static int open_loop(rf_dit* h, const void* pooled, const uint16_t* timesteps_bf16_host, const float* sigmas_host,
+                     int n_steps, float guidance_scale, const void* cond_latents, bool guided,
+                     float image_guidance_scale, cudaStream_t s) {
+  rf::DeviceAllocs& gm = h->geo_mem;
+  const int B = h->batch;
+  // growing keeps the old arrays until the geometry is freed: cudaFree would synchronise the device mid-call
+  if (n_steps > h->tab_steps) {
+    const size_t rows = static_cast<size_t>(B) * n_steps;
+    RF_TRY(gm.alloc(&h->s_tsteps, n_steps));
+    RF_TRY(gm.alloc(&h->s_sigmas, n_steps + 1));
+    RF_TRY(gm.alloc(&h->tab, rows * h->n_mod));
+    RF_TRY(gm.alloc(&h->temb_ws, temb_ws_elems(h, n_steps)));
+    RF_TRY(gm.alloc(&h->idx, rows));
+    h->tab_u = nullptr;
+    std::vector<int> idx(rows);
+    for (size_t r = 0; r < rows; ++r) idx[r] = static_cast<int>(r);
+    RF_CHECK_CUDA(cudaMemcpyAsync(h->idx, idx.data(), rows * sizeof(int), cudaMemcpyHostToDevice, s));
+    h->tab_steps = n_steps;
     drop_graph(h);
   }
+  // no guided step exists without tab_u
+  if (guided && !h->tab_u) RF_TRY(gm.alloc(&h->tab_u, static_cast<size_t>(B) * h->tab_steps * h->n_mod));
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_tsteps, timesteps_bf16_host, static_cast<size_t>(n_steps) * 2,
                                 cudaMemcpyHostToDevice, s));
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_sigmas, sigmas_host, static_cast<size_t>(n_steps + 1) * 4,
@@ -1229,64 +1248,80 @@ static int stage_schedule(rf_dit* h, const uint16_t* timesteps_bf16_host, const 
   RF_CHECK_CUDA(cudaMemcpyAsync(h->s_guid, &gb, 2, cudaMemcpyHostToDevice, s));
   if (guided)
     RF_CHECK_CUDA(cudaMemcpyAsync(h->s_igs, &image_guidance_scale, 4, cudaMemcpyHostToDevice, s));
+  if (h->n_cond > 0)
+    RF_CHECK_CUDA(cudaMemcpyAsync(h->loop_cond, cond_latents,
+                                  static_cast<size_t>(B) * h->n_cond * h->cfg.in_channels * 2,
+                                  cudaMemcpyDeviceToDevice, s));
+  for (int b = 0; b < B; ++b) {
+    const bf16* pool_b = static_cast<const bf16*>(pooled) + static_cast<int64_t>(b) * h->cfg.pooled_projection_dim;
+    const int64_t row0 = static_cast<int64_t>(b) * n_steps * h->n_mod;
+    if (h->n_cond > 0) RF_TRY(compute_cond_mod(h, pool_b, s, h->tab_c + static_cast<int64_t>(b) * h->n_mod));
+    RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, pool_b, (h->flags & 1) != 0, true, h->tab + row0,
+                    h->temb_ws, s));
+    // the uncond branch: guidance = torch.ones_like(guidance) -> bf16(1) * 1000 in the model (generate.py:262)
+    if (guided)
+      RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_zero_one + 1, pool_b, (h->flags & 1) != 0, true,
+                      h->tab_u + row0, h->temb_ws, s));
+  }
+  h->sess_steps = n_steps;
+  h->sess_guided = guided;
+  // the captured step holds the LoRA scalings as kernel parameters (and skips the terms a zero scaling
+  // removes): a changed call scale is re-captured
+  StepGraph* g = guided ? &h->graph_ig : &h->graph;
+  if (g->exec && g->call_scale != h->call_scale) drop_graph(h);
+  if (!g->exec) RF_TRY(capture_step(h, guided, g, s));
   return 0;
 }
 
-// rf_dit_denoise, and with uncond_latents != nullptr rf_dit_denoise_image_guidance (arguments checked by the caller)
-static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
-                        const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
-                        float guidance_scale, const void* cond_latents, const bf16* uncond_latents,
-                        float image_guidance_scale, void* stream) {
-  const bool guided = uncond_latents != nullptr;
+// Step i of sample b of the open loop: stage sample b of latents [B, n_img, C] and txt [B, n_txt, 4096], its condition
+// latents, cond_temb vectors and (image-guided loops) U_i `ucond`, set the sigma index and the table row, replay the
+// captured step and copy the sample's latents back.  Device-to-device copies only.
+static int loop_step(rf_dit* h, int b, int i, void* latents, const void* txt, const bf16* ucond, cudaStream_t s) {
+  const size_t lat_bytes = static_cast<size_t>(h->n_img) * h->cfg.in_channels * 2;
+  const size_t txt_bytes = static_cast<size_t>(h->n_txt) * h->cfg.joint_attention_dim * 2;
+  char* lat = static_cast<char*>(latents) + b * lat_bytes;
+  const size_t cond_elems = static_cast<size_t>(h->n_cond) * h->cfg.in_channels;
+  const size_t mod_bytes = static_cast<size_t>(h->n_mod) * 2;
+  auto d2d = [&](void* dst, const void* src, size_t bytes) {
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
+  };
+  RF_CHECK_CUDA(d2d(h->s_lat, lat, lat_bytes));
+  RF_CHECK_CUDA(d2d(h->s_txt, static_cast<const char*>(txt) + b * txt_bytes, txt_bytes));
+  if (h->n_cond > 0) {
+    RF_CHECK_CUDA(d2d(h->s_cond, h->loop_cond + b * cond_elems, cond_elems * 2));
+    RF_CHECK_CUDA(d2d(h->MODC, h->tab_c + static_cast<int64_t>(b) * h->n_mod, mod_bytes));
+  }
+  if (h->sess_guided) RF_CHECK_CUDA(d2d(h->s_ucond, ucond, cond_elems * 2));
+  RF_CHECK_CUDA(d2d(h->s_step, h->idx + i, sizeof(int)));
+  RF_CHECK_CUDA(d2d(h->s_row, h->idx + b * h->sess_steps + i, sizeof(int)));
+  const StepGraph& g = h->sess_guided ? h->graph_ig : h->graph;
+  RF_CHECK_CUDA(cudaGraphLaunch(g.exec, s));
+  rf::count_launch(static_cast<int>(g.kernels));
+  RF_CHECK_CUDA(d2d(lat, h->s_lat, lat_bytes));
+  return 0;
+}
+
+// rf_dit_denoise and rf_dit_denoise_image_guidance: open the loop, then step 0 .. n_steps-1 of every sample.
+// uncond_latents: [B, n_steps, n_cond, C] (guided).
+static int run_loop(rf_dit* h, const char* who, bool guided, void* latents_inout, const void* txt, const void* pooled,
+                    const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps, float guidance_scale,
+                    const void* cond_latents, const void* uncond_latents, float image_guidance_scale, void* stream) {
   // The loop runs on the handle's side stream, so the step can be captured whatever stream the caller passes
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  const bool inputs_ok = latents_inout && txt && (!guided || (cond_latents && uncond_latents));
+  RF_TRY(check_loop(h, who, caller, inputs_ok, pooled, timesteps_bf16_host, sigmas_host, n_steps, cond_latents,
+                    guided, image_guidance_scale));
   cudaStream_t s = nullptr;
   RF_TRY(h->side.enter(caller, &s));
-  h->sess = false;  // this loop rewrites the step's staging and tables
-  const int C = h->cfg.in_channels;
-  RF_TRY(stage_schedule(h, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, guided, image_guidance_scale, s));
-  StepGraph* g = guided ? &h->graph_ig : &h->graph;
-  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
-
-  for (int b = 0; b < h->batch; ++b) {
-    bf16* lat_b = static_cast<bf16*>(latents_inout) + static_cast<int64_t>(b) * h->n_img * C;
-    // stage this sample's inputs so the captured graph always sees the same addresses
-    RF_CHECK_CUDA(cudaMemcpyAsync(h->s_lat, lat_b, static_cast<size_t>(h->n_img) * C * 2,
-                                  cudaMemcpyDeviceToDevice, s));
-    RF_CHECK_CUDA(cudaMemcpyAsync(
-        h->s_txt,
-        static_cast<const bf16*>(txt) + static_cast<int64_t>(b) * h->n_txt * h->cfg.joint_attention_dim,
-        static_cast<size_t>(h->n_txt) * h->cfg.joint_attention_dim * 2, cudaMemcpyDeviceToDevice, s));
-    RF_CHECK_CUDA(cudaMemcpyAsync(
-        h->s_pooled,
-        static_cast<const bf16*>(pooled) + static_cast<int64_t>(b) * h->cfg.pooled_projection_dim,
-        static_cast<size_t>(h->cfg.pooled_projection_dim) * 2, cudaMemcpyDeviceToDevice, s));
-    if (h->n_cond > 0) {
-      RF_CHECK_CUDA(cudaMemcpyAsync(
-          h->s_cond, static_cast<const bf16*>(cond_latents) + static_cast<int64_t>(b) * h->n_cond * C,
-          static_cast<size_t>(h->n_cond) * C * 2, cudaMemcpyDeviceToDevice, s));
-      RF_TRY(compute_cond_mod(h, h->s_pooled, s));  // hoisted out of the step loop
+  RF_TRY(open_loop(h, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, cond_latents, guided,
+                   image_guidance_scale, s));
+  const int64_t cond_elems = static_cast<int64_t>(h->n_cond) * h->cfg.in_channels;
+  for (int i = 0; i < n_steps; ++i) {
+    for (int b = 0; b < h->batch; ++b) {
+      const int64_t u = (static_cast<int64_t>(b) * n_steps + i) * cond_elems;  // U_i of sample b
+      const bf16* ucond = guided ? static_cast<const bf16*>(uncond_latents) + u : nullptr;
+      RF_TRY(loop_step(h, b, i, latents_inout, txt, ucond, s));
     }
-    RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, h->s_pooled, (h->flags & 1) != 0, true, h->s_mod_all,
-                    h->s_temb_ws, s));
-    // the uncond branch: guidance = torch.ones_like(guidance) -> bf16(1) * 1000 in the model (generate.py:262)
-    if (guided)
-      RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_zero_one + 1, h->s_pooled, (h->flags & 1) != 0, true,
-                      h->s_mod_all_u, h->s_temb_ws, s));
-    RF_CHECK_CUDA(cudaMemsetAsync(h->s_step, 0, sizeof(int), s));
-    // the captured step holds the LoRA scalings as kernel parameters (and skips the terms a zero scaling
-    // removes): a changed call scale is re-captured
-    if (g->exec && g->call_scale != h->call_scale) drop_graph(h);
-    if (!g->exec) RF_TRY(capture_step(h, guided, g, s));
-    for (int i = 0; i < n_steps; ++i) {
-      if (guided)  // U_i of this sample: [B, n_steps, n_cond, 64]
-        RF_CHECK_CUDA(cudaMemcpyAsync(h->s_ucond, uncond_latents + (static_cast<size_t>(b) * n_steps + i) * cond_elems,
-                                      cond_elems * 2, cudaMemcpyDeviceToDevice, s));
-      RF_CHECK_CUDA(cudaGraphLaunch(g->exec, s));
-      rf::count_launch(static_cast<int>(g->kernels));
-    }
-    RF_CHECK_CUDA(cudaMemcpyAsync(lat_b, h->s_lat, static_cast<size_t>(h->n_img) * C * 2,
-                                  cudaMemcpyDeviceToDevice, s));
   }
   return h->side.leave(caller);
 }
@@ -1294,108 +1329,30 @@ static int denoise_loop(rf_dit* h, void* latents_inout, const void* txt, const v
 int rf_dit_denoise(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
                    const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
                    float guidance_scale, const void* cond_latents, void* stream) {
-  int rc = check_ready(h, "rf_dit_denoise", static_cast<cudaStream_t>(stream));
-  if (rc) return rc;
-  if (!latents_inout || !txt || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 ||
-      (h->n_cond > 0 && !cond_latents)) {
-    rf::set_error("rf_dit_denoise: bad argument");
-    return -1;
-  }
-  return denoise_loop(h, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale,
-                      cond_latents, nullptr, 1.0f, stream);
+  return run_loop(h, "rf_dit_denoise", false, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps,
+                  guidance_scale, cond_latents, nullptr, 1.0f, stream);
 }
 
 int rf_dit_denoise_image_guidance(rf_dit* h, void* latents_inout, const void* txt, const void* pooled,
                                   const uint16_t* timesteps_bf16_host, const float* sigmas_host, int n_steps,
                                   float guidance_scale, const void* cond_latents, const void* uncond_latents,
                                   float image_guidance_scale, void* stream) {
-  int rc = check_ready(h, "rf_dit_denoise_image_guidance", static_cast<cudaStream_t>(stream));
-  if (rc) return rc;
-  if (!latents_inout || !txt || !pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 || !cond_latents ||
-      !uncond_latents) {
-    rf::set_error("rf_dit_denoise_image_guidance: bad argument");
-    return -1;
-  }
-  if (h->n_cond <= 0 || !h->cfg.guidance_embeds) {
-    rf::set_error("rf_dit_denoise_image_guidance: needs a condition stream (n_cond > 0) and guidance_embeds");
-    return -1;
-  }
-  if (!std::isfinite(image_guidance_scale)) {
-    rf::set_error("rf_dit_denoise_image_guidance: image_guidance_scale must be finite");
-    return -1;
-  }
-  return denoise_loop(h, latents_inout, txt, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale,
-                      cond_latents, static_cast<const bf16*>(uncond_latents), image_guidance_scale, stream);
+  return run_loop(h, "rf_dit_denoise_image_guidance", true, latents_inout, txt, pooled, timesteps_bf16_host,
+                  sigmas_host, n_steps, guidance_scale, cond_latents, uncond_latents, image_guidance_scale, stream);
 }
 
 int rf_dit_denoise_begin(rf_dit* h, const void* pooled, const uint16_t* timesteps_bf16_host, const float* sigmas_host,
                          int n_steps, float guidance_scale, const void* cond_latents, float image_guidance_scale,
                          void* stream) {
-  int rc = check_ready(h, "rf_dit_denoise_begin", static_cast<cudaStream_t>(stream));
-  if (rc) return rc;
-  h->sess = false;
-  if (!pooled || !timesteps_bf16_host || !sigmas_host || n_steps <= 0 || (h->n_cond > 0 && !cond_latents)) {
-    rf::set_error("rf_dit_denoise_begin: bad argument");
-    return -1;
-  }
-  const bool guided = image_guidance_scale != 1.0f;
-  if (guided && (h->n_cond <= 0 || !h->cfg.guidance_embeds)) {
-    rf::set_error("rf_dit_denoise_begin: image_guidance_scale != 1 needs a condition stream (n_cond > 0) and "
-                  "guidance_embeds");
-    return -1;
-  }
-  if (!std::isfinite(image_guidance_scale)) {
-    rf::set_error("rf_dit_denoise_begin: image_guidance_scale must be finite");
-    return -1;
-  }
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  const bool guided = image_guidance_scale != 1.0f;
+  RF_TRY(check_loop(h, "rf_dit_denoise_begin", caller, true, pooled, timesteps_bf16_host, sigmas_host, n_steps,
+                    cond_latents, guided, image_guidance_scale));
   cudaStream_t s = nullptr;
   RF_TRY(h->side.enter(caller, &s));
-  const int C = h->cfg.in_channels, B = h->batch;
-  RF_TRY(stage_schedule(h, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, guided, image_guidance_scale, s));
-  rf::DeviceAllocs& gm = h->geo_mem;
-  const int64_t rows = static_cast<int64_t>(B) * n_steps;
-  if (rows > h->sess_rows) {
-    gm.release(h->sess_mod);
-    RF_TRY(gm.alloc(&h->sess_mod, static_cast<size_t>(rows) * h->n_mod));
-    h->sess_rows = rows;
-  }
-  if (guided && rows > h->sess_rows_u) {
-    gm.release(h->sess_mod_u);
-    RF_TRY(gm.alloc(&h->sess_mod_u, static_cast<size_t>(rows) * h->n_mod));
-    h->sess_rows_u = rows;
-  }
-  if (n_steps > h->sess_idx_n) {
-    gm.release(h->sess_idx);
-    RF_TRY(gm.alloc(&h->sess_idx, n_steps));
-    std::vector<int> idx(n_steps);
-    for (int i = 0; i < n_steps; ++i) idx[i] = i;
-    RF_CHECK_CUDA(cudaMemcpyAsync(h->sess_idx, idx.data(), static_cast<size_t>(n_steps) * 4, cudaMemcpyHostToDevice, s));
-    h->sess_idx_n = n_steps;
-  }
-  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
-  if (h->n_cond > 0) {
-    if (!h->sess_modc) RF_TRY(gm.alloc(&h->sess_modc, static_cast<size_t>(B) * h->n_mod));
-    if (!h->sess_cond) RF_TRY(gm.alloc(&h->sess_cond, B * cond_elems));
-    RF_CHECK_CUDA(cudaMemcpyAsync(h->sess_cond, cond_latents, B * cond_elems * 2, cudaMemcpyDeviceToDevice, s));
-  }
-  // the tables of every sample, by the same temb_mod calls as the whole loop: bit-identical rows
-  for (int b = 0; b < B; ++b) {
-    const bf16* pool_b = static_cast<const bf16*>(pooled) + static_cast<int64_t>(b) * h->cfg.pooled_projection_dim;
-    const int64_t row0 = static_cast<int64_t>(b) * n_steps * h->n_mod;
-    if (h->n_cond > 0) RF_TRY(compute_cond_mod(h, pool_b, s, h->sess_modc + static_cast<int64_t>(b) * h->n_mod));
-    RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_guid, pool_b, (h->flags & 1) != 0, true, h->sess_mod + row0,
-                    h->s_temb_ws, s));
-    if (guided)
-      RF_TRY(temb_mod(h, n_steps, h->s_tsteps, h->s_zero_one + 1, pool_b, (h->flags & 1) != 0, true,
-                      h->sess_mod_u + row0, h->s_temb_ws, s));
-  }
-  StepGraph* g = guided ? &h->graph_ig : &h->graph;
-  if (g->exec && g->call_scale != h->call_scale) drop_graph(h);
-  if (!g->exec) RF_TRY(capture_step(h, guided, g, s));
+  RF_TRY(open_loop(h, pooled, timesteps_bf16_host, sigmas_host, n_steps, guidance_scale, cond_latents, guided,
+                   image_guidance_scale, s));
   h->sess = true;
-  h->sess_guided = guided;
-  h->sess_steps = n_steps;
   return h->side.leave(caller);
 }
 
@@ -1423,35 +1380,10 @@ int rf_dit_denoise_step(rf_dit* h, int i, void* latents_inout, const void* txt, 
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
   cudaStream_t s = nullptr;
   RF_TRY(h->side.enter(caller, &s));
-  const int C = h->cfg.in_channels;
-  const size_t lat_bytes = static_cast<size_t>(h->n_img) * C * 2;
-  const size_t txt_elems = static_cast<size_t>(h->n_txt) * h->cfg.joint_attention_dim;
-  const size_t cond_elems = static_cast<size_t>(h->n_cond) * C;
-  const size_t mod_bytes = static_cast<size_t>(h->n_mod) * 2;
-  const StepGraph* g = h->sess_guided ? &h->graph_ig : &h->graph;
-  auto d2d = [&](void* dst, const void* src, size_t bytes) {
-    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
-  };
+  const int64_t cond_elems = static_cast<int64_t>(h->n_cond) * h->cfg.in_channels;
   for (int b = 0; b < h->batch; ++b) {
-    bf16* lat_b = static_cast<bf16*>(latents_inout) + static_cast<int64_t>(b) * h->n_img * C;
-    const int64_t row = static_cast<int64_t>(b) * h->sess_steps + i;
-    RF_CHECK_CUDA(d2d(h->s_lat, lat_b, lat_bytes));
-    RF_CHECK_CUDA(d2d(h->s_txt, static_cast<const bf16*>(txt) + b * txt_elems, txt_elems * 2));
-    // the captured step selects row *s_step of s_mod_all: put sample b's row i there
-    RF_CHECK_CUDA(d2d(h->s_mod_all + static_cast<int64_t>(i) * h->n_mod, h->sess_mod + row * h->n_mod, mod_bytes));
-    if (h->n_cond > 0) {
-      RF_CHECK_CUDA(d2d(h->s_cond, h->sess_cond + b * cond_elems, cond_elems * 2));
-      RF_CHECK_CUDA(d2d(h->MODC, h->sess_modc + static_cast<int64_t>(b) * h->n_mod, mod_bytes));
-    }
-    if (h->sess_guided) {
-      RF_CHECK_CUDA(d2d(h->s_mod_all_u + static_cast<int64_t>(i) * h->n_mod, h->sess_mod_u + row * h->n_mod,
-                        mod_bytes));
-      RF_CHECK_CUDA(d2d(h->s_ucond, static_cast<const bf16*>(uncond_latents_i) + b * cond_elems, cond_elems * 2));
-    }
-    RF_CHECK_CUDA(d2d(h->s_step, h->sess_idx + i, sizeof(int)));
-    RF_CHECK_CUDA(cudaGraphLaunch(g->exec, s));
-    rf::count_launch(static_cast<int>(g->kernels));
-    RF_CHECK_CUDA(d2d(lat_b, h->s_lat, lat_bytes));
+    const bf16* ucond = h->sess_guided ? static_cast<const bf16*>(uncond_latents_i) + b * cond_elems : nullptr;
+    RF_TRY(loop_step(h, b, i, latents_inout, txt, ucond, s));
   }
   return h->side.leave(caller);
 }

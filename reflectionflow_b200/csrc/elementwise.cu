@@ -393,17 +393,6 @@ int image_guidance_step_launch(bf16* x, const bf16* v_cond, const bf16* v_uncond
   return 0;
 }
 
-__global__ void advance_step_kernel(int* step) {
-  pdl_launch_dependents();
-  pdl_wait();
-  *step += 1;
-}
-int advance_step_launch(int* step, cudaStream_t stream) {
-  RF_CHECK_CUDA(launch_pdl(advance_step_kernel, dim3(1), dim3(1), 0, stream, step));
-  count_launch();
-  return 0;
-}
-
 __global__ void copy_rows_kernel(const bf16* __restrict__ src, int lds, bf16* __restrict__ dst,
                                  int ldd, int rows, int chunks_per_row) {
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;

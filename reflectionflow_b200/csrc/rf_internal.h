@@ -254,7 +254,6 @@ int gemv_launch(const bf16* x, int ldx, int batch, const bf16* W, const bf16* bi
 //   t value of batch b = t[b * t_stride + (step ? *step : 0)]
 int timestep_embed_launch(const bf16* t, const int* step, int t_stride, float pre_scale, bf16* out,
                           int batch, cudaStream_t stream);
-int advance_step_launch(int* step, cudaStream_t stream);
 // out = bf16(a + b + c) evaluated left to right with bf16 rounding after each add
 int add3_launch(const bf16* a, const bf16* b, const bf16* c, bf16* out, int n,
                 cudaStream_t stream);

@@ -236,10 +236,10 @@ def test_refusals():
         m.close()
 
 
-def test_guided_step_launches_two_forwards_and_two_kernels():
-    """Per extra step, the plain loop runs its captured step (F + 2 launches: forward, Euler, counter) plus one add
-    of the step's modulation table; the guided loop runs its step (2 F + 2: two forwards, guidance + Euler,
-    counter) plus one add of each of its two tables."""
+def test_guided_step_launches_two_forwards_and_one_kernel():
+    """Per extra step, the plain loop runs its captured step (F + 1 launches: forward, Euler) plus one add of the
+    step's modulation table; the guided loop runs its step (2 F + 1: two forwards, guidance + Euler) plus one add of
+    each of its two tables."""
     lib = L.load()
     m = _model(SMALL)
     try:
@@ -256,6 +256,6 @@ def test_guided_step_launches_two_forwards_and_two_kernels():
         guided_step = per_step(1.5) - 2
     finally:
         m.close()
-    forward = plain_step - 2
+    forward = plain_step - 1
     assert forward > 10
-    assert guided_step == 2 * forward + 2, (plain_step, guided_step)
+    assert guided_step == 2 * forward + 1, (plain_step, guided_step)
